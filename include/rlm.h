@@ -269,6 +269,15 @@ int rlm_test_to_ticks(const rlm_config* cfg, const double* px, int32_t n, int32_
 int rlm_test_to_price(const rlm_config* cfg, const int32_t* ticks, int32_t n, double* out);
 /* tiles() (src/rl/tiles.cpp:31-75) for n states of n_vars floats, all actions: out[n][n_actions][96] */
 int rlm_test_tiles(const rlm_config* cfg, const float* vars, int32_t n, int32_t* out);
+/* TEST ONLY.  The same tile indices as each learner kernel derives them (cfg sets memory_size, n_actions, n_state_vars):
+ *   RLM_TILES_THREE_WARP    tile_base_sum + tile_index (rlm_agent3_kernel, round-1 kernels)      out[n][n_actions][96]
+ *   RLM_TILES_ONE_WARP      ln_hash + ln_tile (rlm_learn_kernel, the fused 'F' engine)           out[n][n_actions][96]
+ *   RLM_TILES_STAGED        the 16-bit index rows of rlm_learn_staged_kernel (memory_size <= 8192) out[n][n_actions][96]
+ *   RLM_TILES_TRACE_GROUP0  group 0 rebuilt from the stored base (base mod M + action term) mod M, as the trace passes
+ *                           and tile tables do                                                    out[n][n_actions][32]
+ * Writes only `out`.  Returns RLM_ERR_UNSUPPORTED for RLM_TILES_STAGED above 8192. */
+enum { RLM_TILES_THREE_WARP = 0, RLM_TILES_ONE_WARP = 1, RLM_TILES_STAGED = 2, RLM_TILES_TRACE_GROUP0 = 3 };
+int rlm_test_learner_tiles(const rlm_config* cfg, int32_t form, const float* vars, int32_t n, int32_t* out);
 /* Order script (test/test_Order.cpp): op codes see rlm_order_op */
 typedef struct rlm_order_op { int32_t op; int32_t pad; int64_t arg; } rlm_order_op; /* 0=doTransaction 1=doCancellation 2=addVolumeBehind 3=clearQueues */
 typedef struct rlm_order_state { int64_t size, q_head, q_tail, executed, ret; } rlm_order_state;

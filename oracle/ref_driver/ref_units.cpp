@@ -129,26 +129,56 @@ int main() {
   printf("],\n");
 
   // ---------------------------------------------------------------- tiles via rl::State (src/rl/state.cpp:53-65)
+  // One entry per (memory_size, n_actions, n_vars); features[a*96 + i] = State::getFeatures(a)[i].
   printf("\"tiles\": [\n");
+  auto tile_entry = [](long mem, int n_actions, int n_vars, const vector<vector<float>>& states, bool last) {
+    rl::State st(mem, n_actions, 32);
+    printf("  {\"memory_size\": %ld, \"n_actions\": %d, \"n_vars\": %d, \"cases\": [\n", mem, n_actions, n_vars);
+    for (size_t k = 0; k < states.size(); ++k) {
+      vector<float> v = states[k];
+      st.newState(v, 0.0);
+      printf("    {\"vars\": [");
+      for (int i = 0; i < n_vars; ++i) { uint32_t u; memcpy(&u, &v[i], 4); printf("%s%u", i ? ", " : "", u); }
+      printf("], \"features\": [");
+      for (int a = 0; a < n_actions; ++a) {
+        auto& f = st.getFeatures(a);
+        for (int i = 0; i < 96; ++i) printf("%s%d", (a || i) ? ", " : "", f[i]);
+      }
+      printf("]}%s\n", k + 1 < states.size() ? "," : "");
+    }
+    printf("  ]}%s\n", last ? "" : ",");
+  };
   long mems[3] = {65536, 20000000, 5003};
   for (int mi = 0; mi < 3; ++mi) {
-    rl::State st(mems[mi], 9, 32);
-    printf("  {\"memory_size\": %ld, \"cases\": [\n", mems[mi]);
+    vector<vector<float>> states;
     for (int k = 0; k < 6; ++k) {
       vector<float> v(8);
       if (k == 0) v = {0.5f, -100.0f, -100.0f, 0.0f, 1.0f, 0.0f, 0.0f, 0.0f};
       else for (int i = 0; i < 8; ++i) v[i] = (float)((int)(lcg() % 4000) - 2000) / 97.0f;
-      st.newState(v, 0.0);
-      printf("    {\"vars\": [");
-      for (int i = 0; i < 8; ++i) { uint32_t u; memcpy(&u, &v[i], 4); printf("%s%u", i ? ", " : "", u); }
-      printf("], \"features\": [");
-      for (int a = 0; a < 9; ++a) {
-        auto& f = st.getFeatures(a);
-        for (int i = 0; i < 96; ++i) printf("%s%d", (a || i) ? ", " : "", f[i]);
-      }
-      printf("]}%s\n", k < 5 ? "," : "");
+      states.push_back(v);
     }
-    printf("  ]}%s\n", mi < 2 ? "," : "");
+    tile_entry(mems[mi], 9, 8, states, false);
+  }
+  // The edges of the learner's index arithmetic: tables smaller than a step's 32 tiles per group (M = 1 has no
+  // magic-number reciprocal; 1 and 2 are powers of two), both sides of the 2^27 limit of the packed tile table, and
+  // tables above 2^30, where the sum of two indices below M no longer fits an int.  Every action count meets every
+  // state size over the sweep.  A generator of its own keeps the vectors of the other sections as they were.
+  {
+    uint64_t s = 977;
+    auto next = [&s]() -> uint32_t { s = s * 6364136223846793005ull + 1442695040888963407ull; return (uint32_t)(s >> 33); };
+    const long edge[8] = {1, 2, 3, 1L << 27, (1L << 27) + 1, (1L << 30) + 3, 3L << 29, 2147483647L};
+    const int acts[3] = {1, 5, 9}, nvars[3] = {4, 8, 13};
+    for (int mi = 0; mi < 8; ++mi)
+      for (int c = 0; c < 3; ++c) {
+        const int nv = nvars[(c + mi) % 3];
+        vector<vector<float>> states;
+        for (int k = 0; k < 2; ++k) {
+          vector<float> v(nv);
+          for (int i = 0; i < nv; ++i) v[i] = (float)((int)(next() % 40000) - 20000) / 97.0f;
+          states.push_back(v);
+        }
+        tile_entry(edge[mi], acts[c], nv, states, mi == 7 && c == 2);
+      }
   }
   printf("],\n");
 

@@ -142,6 +142,13 @@ __device__ __noinline__ unsigned long long tile_base_sum(const unsigned* rnd, co
 __device__ __forceinline__ int tile_index(const unsigned* rnd, unsigned long long base, int nf, int h1) {
   return mod_m(base + __ldg(rnd + ((h1 + 449 * (nf + 1)) & 2047)));
 }
+// group-0 tile of action a from a stored base b0 = (partial hash sum) mod M: (b0 + ra_m[a]) mod M.  Both terms are below
+// M <= 2^31 - 1, so their sum can pass INT_MAX once M > 2^30: it is formed unsigned (< 2^32) and reduced by one subtract.
+__device__ __forceinline__ int tile0_from_base(int b0, int a) {
+  unsigned f = (unsigned)b0 + (unsigned)P.ra_m[a];
+  if (f >= (unsigned)P.memory_size) f -= (unsigned)P.memory_size;
+  return (int)f;
+}
 
 // ---- tile hashing of one state.  sums[g] = lane's partial hash sum of group g (everything but the action term);
 // tile (group g, tiling `lane`, action a) = (sums[g] + rg[g][a]) mod M.  The sums are what stays live across the step
@@ -441,9 +448,7 @@ __device__ __forceinline__ void tt_fill(int* tt, const AgentD& e, int t, int n_t
   const int n = P.n_actions * 32;
   for (int i = t; i < n; i += n_threads) {
     const int a = i >> 5, j = i & 31;
-    int f = e.from_base0[j] + P.ra_m[a];
-    if (f >= (int)P.memory_size) f -= (int)P.memory_size;
-    tt_insert(tt, f, a);
+    tt_insert(tt, tile0_from_base(e.from_base0[j], a), a);
   }
 }
 
@@ -534,11 +539,7 @@ __device__ __noinline__ int trace_pass(AgentD& e, int* ss, const int* tt, int* t
   TP(2);
   // set(): the taken action's tiles that no later action cleared; one entry per distinct f
   {
-    int f = 0;
-    if (!null_from) {
-      f = b0 + P.ra_m[action];
-      if (f >= (int)P.memory_size) f -= (int)P.memory_size;
-    }
+    const int f = null_from ? 0 : tile0_from_base(b0, action);
     // f is a tile of `action` by construction: only later actions can still clear it
     bool add;
     if (null_from) add = (action == P.n_actions - 1);

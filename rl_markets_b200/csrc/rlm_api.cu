@@ -1330,6 +1330,22 @@ int rlm_test_tiles(const rlm_config* cfg, const float* vars, int32_t n, int32_t*
   cudaFree(d_in); cudaFree(d_out);
   return RLM_OK;
 }
+int rlm_test_learner_tiles(const rlm_config* cfg, int32_t form, const float* vars, int32_t n, int32_t* out) {
+  API_LOCK;
+  if (form < RLM_TILES_THREE_WARP || form > RLM_TILES_TRACE_GROUP0) return fail(RLM_ERR_INVALID_ARGUMENT, "unknown tile form");
+  if (form == RLM_TILES_STAGED && cfg->memory_size > 8192) return fail(RLM_ERR_UNSUPPORTED, "the staged learner holds tables of at most 8192 weights");
+  rlm_handle_s tmp;
+  int rc = test_setup(cfg, tmp);
+  if (rc) return rc;
+  float* d_in; int* d_out;
+  size_t nin = (size_t)n * cfg->n_state_vars, nout = (size_t)n * cfg->n_actions * (form == RLM_TILES_TRACE_GROUP0 ? 32 : 96);
+  CK(cudaMalloc(&d_in, nin * 4)); CK(cudaMalloc(&d_out, nout * 4));
+  CK(cudaMemcpy(d_in, vars, nin * 4, cudaMemcpyHostToDevice));
+  CK(rlm_launch_test_learner_tiles(form, d_in, n, d_out));
+  CK(cudaMemcpy(out, d_out, nout * 4, cudaMemcpyDeviceToHost));
+  cudaFree(d_in); cudaFree(d_out);
+  return RLM_OK;
+}
 int rlm_test_order(int64_t size, int64_t q_head, const rlm_order_op* ops, int32_t n_ops, rlm_order_state* out) {
   API_LOCK;
   int ndev = 0;

@@ -2109,6 +2109,35 @@ __global__ void k_test_tiles(const float* vars, int n, int* out) {
     for (int a = 0; a < A; ++a) out[((size_t)warp * A + a) * 96 + g * 32 + lane] = tile_index(s_rnd, base, nf, g * A + a);
   }
 }
+// one warp per state: the tile indices as each learner form derives them (rlm_test_learner_tiles in include/rlm.h)
+__global__ void k_test_learner_tiles(int form, const float* vars, int n, int* out) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= n) return;
+  const float* v = vars + (size_t)warp * P.n_state_vars;
+  const int A = P.n_actions;
+  if (form == RLM_TILES_THREE_WARP) {
+    for (int g = 0; g < 3; ++g) {
+      const float* gv = (g == 1) ? v + 3 : v;
+      const int nf = (g == 0) ? 3 : ((g == 1) ? P.n_state_vars - 3 : P.n_state_vars);
+      const unsigned long long base = tile_base_sum(rlm_rndseq_table, gv, nf, lane);
+      for (int a = 0; a < A; ++a) out[((size_t)warp * A + a) * 96 + g * 32 + lane] = tile_index(rlm_rndseq_table, base, nf, g * A + a);
+    }
+    return;
+  }
+  const LnSums h = ln_hash(rlm_rndseq_table, v, false, lane);
+  if (form == RLM_TILES_TRACE_GROUP0) {  // EnvHdr::from_base0 and the group-0 tile rebuilt from it (trace passes, tile tables)
+    const int b0 = mod_m(h.s[0]);
+    for (int a = 0; a < A; ++a) out[((size_t)warp * A + a) * 32 + lane] = tile0_from_base(b0, a);
+    return;
+  }
+  for (int k = 0; k < 3 * RLM_MAX_ACTIONS; ++k) {
+    const int g = k / RLM_MAX_ACTIONS, a = k % RLM_MAX_ACTIONS;
+    if (a >= A) continue;
+    int f = P.m_pow2 ? ln_tile<true>(h, k) : ln_tile<false>(h, k);  // rlm_learn_kernel's gathers and ln_patch_local
+    if (form == RLM_TILES_STAGED) f = (unsigned short)f;            // rlm_learn_staged_kernel's 16-bit index rows
+    out[((size_t)warp * A + a) * 96 + g * 32 + lane] = f;
+  }
+}
 __global__ void k_test_order(long long size, long long q_head, const rlm_order_op* ops, int n_ops, rlm_order_state* out) {
   if (threadIdx.x || blockIdx.x) return;
   OrderD o; o.live = 1; o.price = 1.0; o.size = size; o.q_head = q_head; o.q_tail = 0; o.executed = 0; o.initial_queue = q_head; o.transactions = 0;
@@ -2136,5 +2165,9 @@ __global__ void k_test_rolling_mean(const double* vals, int n, double* out, doub
 cudaError_t rlm_launch_test_to_ticks(const double* px, int n, int* out) { k_test_to_ticks<<<(n + 127) / 128, 128>>>(px, n, out); return cudaGetLastError(); }
 cudaError_t rlm_launch_test_to_price(const int* t, int n, double* out) { k_test_to_price<<<(n + 127) / 128, 128>>>(t, n, out); return cudaGetLastError(); }
 cudaError_t rlm_launch_test_tiles(const float* vars, int n, int* out) { k_test_tiles<<<(n + 3) / 4, 128>>>(vars, n, out); return cudaGetLastError(); }
+cudaError_t rlm_launch_test_learner_tiles(int form, const float* vars, int n, int* out) {
+  k_test_learner_tiles<<<(n + 3) / 4, 128>>>(form, vars, n, out);
+  return cudaGetLastError();
+}
 cudaError_t rlm_launch_test_order(long long size, long long q_head, const rlm_order_op* ops, int n_ops, rlm_order_state* out) { k_test_order<<<1, 32>>>(size, q_head, ops, n_ops, out); return cudaGetLastError(); }
 cudaError_t rlm_launch_test_rolling_mean(const double* vals, int n, double* out, double* ring_mem, EnvHdr* e) { k_test_rolling_mean<<<1, 32>>>(vals, n, out, ring_mem, e); return cudaGetLastError(); }

@@ -33,5 +33,6 @@ cudaError_t rlm_launch_clear_traces(const DevPtrs& ptr, int n_envs, cudaStream_t
 cudaError_t rlm_launch_test_to_ticks(const double* px, int n, int* out);
 cudaError_t rlm_launch_test_to_price(const int* t, int n, double* out);
 cudaError_t rlm_launch_test_tiles(const float* vars, int n, int* out);
+cudaError_t rlm_launch_test_learner_tiles(int form, const float* vars, int n, int* out);
 cudaError_t rlm_launch_test_order(long long size, long long q_head, const rlm_order_op* ops, int n_ops, rlm_order_state* out);
 cudaError_t rlm_launch_test_rolling_mean(const double* vals, int n, double* out, double* ring_mem, EnvHdr* e);

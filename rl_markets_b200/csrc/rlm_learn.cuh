@@ -234,13 +234,8 @@ __device__ __forceinline__ void ln_tt_build(int* tt, const AgentD& ag, int lane)
   __syncwarp();
   if (!ag.null_from) {
     const int b0 = ag.from_base0[lane];
-    const int M = (int)P.memory_size;
 #pragma unroll 1
-    for (int a = 0; a < P.n_actions; ++a) {
-      int f = b0 + P.ra_m[a];
-      if (f >= M) f -= M;
-      ptt_insert(tt, f, a);
-    }
+    for (int a = 0; a < P.n_actions; ++a) ptt_insert(tt, tile0_from_base(b0, a), a);
   }
   __syncwarp();
 }
@@ -292,11 +287,7 @@ __device__ __forceinline__ int ln_trace_pass(AgentD& e, const int* tt, int* ut, 
     }
   }
   {  // set(): the taken action's tiles that no later action cleared; one entry per distinct f
-    int f = 0;
-    if (!null_from) {
-      f = b0 + P.ra_m[action];
-      if (f >= (int)P.memory_size) f -= (int)P.memory_size;
-    }
+    const int f = null_from ? 0 : tile0_from_base(b0, action);
     bool add = null_from ? (action == P.n_actions - 1) : (ptt_last_writer(tt, f) == action);
     const unsigned same = __match_any_sync(FULL, f);
     add = add && ((__ffs(same) - 1) == lane);
@@ -908,11 +899,7 @@ __global__ void __launch_bounds__(32, 6) rlm_learn_staged_kernel(DevPtrs ptr, Dy
         }
       }
       {
-        int f = 0;
-        if (!null_from) {
-          f = ag.from_base0[lane] + P.ra_m[action];
-          if (f >= (int)P.memory_size) f -= (int)P.memory_size;
-        }
+        const int f = null_from ? 0 : tile0_from_base(ag.from_base0[lane], action);
         bool add = null_from ? (action == A - 1) : (ptt_last_writer(tt, f) == action);
         const unsigned same = __match_any_sync(FULL, f);
         add = add && ((__ffs(same) - 1) == lane);

@@ -18,7 +18,7 @@ EXPORTS = [
     "rlm_get_reward", "rlm_get_actions", "rlm_get_rho", "rlm_get_occupancy", "rlm_copy_theta", "rlm_handle_terminal", "rlm_go_greedy", "rlm_read_theta",
     "rlm_write_theta", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
     "rlm_set_stream", "rlm_set_profiling", "rlm_get_kernel_times", "rlm_act", "rlm_env_step", "rlm_agent_update", "rlm_ingest_csv",
-    "rlm_flow_generate", "rlm_test_to_ticks", "rlm_test_to_price", "rlm_test_tiles", "rlm_test_order",
+    "rlm_flow_generate", "rlm_test_to_ticks", "rlm_test_to_price", "rlm_test_tiles", "rlm_test_learner_tiles", "rlm_test_order",
     "rlm_test_rolling_mean",
 ]
 
@@ -80,6 +80,7 @@ def load():
     L.rlm_test_to_ticks.argtypes = [P(abi.Config), P(C.c_double), C.c_int32, P(C.c_int32)]
     L.rlm_test_to_price.argtypes = [P(abi.Config), P(C.c_int32), C.c_int32, P(C.c_double)]
     L.rlm_test_tiles.argtypes = [P(abi.Config), P(C.c_float), C.c_int32, P(C.c_int32)]
+    L.rlm_test_learner_tiles.argtypes = [P(abi.Config), C.c_int32, P(C.c_float), C.c_int32, P(C.c_int32)]
     L.rlm_test_order.argtypes = [C.c_int64, C.c_int64, P(abi.OrderOp), C.c_int32, P(abi.OrderState)]
     L.rlm_test_rolling_mean.argtypes = [C.c_int32, P(C.c_double), C.c_int32, P(C.c_double)]
     _lib = L

@@ -72,6 +72,22 @@ def case_config(case, n_envs=1, env_index0=0, source=abi.SOURCE_GENERATOR):
     return config.from_dict(case["yaml"], n_envs=n_envs, env_index0=env_index0, flow_seed=case["flow_seed"], source=source)
 
 
+_TILE_VARS = ["pos", "spd", "mpm", "imb", "svl", "vol", "rsi", "vwap", "a_dist", "a_queue", "b_dist", "b_queue", "last_action"]
+
+
+def tile_config(entry):
+    """Config of a units.json tile entry: its memory_size, n_actions and number of state variables (which variables
+    they are does not enter tiles(): only their values do)."""
+    y = config.example_dict(**{"learning.memory_size": entry["memory_size"], "learning.n_actions": entry["n_actions"],
+                               "state.variables": _TILE_VARS[:entry["n_vars"]]})
+    return config.from_dict(y)
+
+
+def tile_vars(case):
+    """The state of a units.json tile case as a ctypes float array (stored as bit patterns)."""
+    return (C.c_float * len(case["vars"]))(*[C.c_float.from_buffer_copy(C.c_uint32(u)).value for u in case["vars"]])
+
+
 def hex_to_double(h):
     return struct.unpack("<d", struct.pack("<Q", int(h, 16)))[0]
 

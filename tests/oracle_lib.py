@@ -115,8 +115,10 @@ def generate_ticks(cfg, env_index, n_ticks):
     return arr
 
 
-def run_port(cfg, env_index, ticks, max_steps=-1, rec_cap=None):
-    """Run the CPU restatement for one env; returns (records list, steps, consumed, handle-free stats)."""
+def run_port(cfg, env_index, ticks, max_steps=-1, rec_cap=None, theta_at=None):
+    """Run the CPU restatement for one env; returns (records list, steps, consumed, handle-free stats).
+    theta: the whole table up to 2^20 weights, None above.  theta_nz: (indices, values) of the nonzero weights as
+    numpy arrays, at any size.  theta_at: optional int64 indices whose weights come back as "theta_at"."""
     L = lib()
     h = L.lobo_create(C.byref(cfg), env_index)
     assert h, "lobo_create failed"
@@ -133,6 +135,13 @@ def run_port(cfg, env_index, ticks, max_steps=-1, rec_cap=None):
     M = cfg.memory_size
     th = L.lobo_theta(h, 0)
     out["theta"] = [th[i] for i in range(M)] if M <= (1 << 20) else None
+    import numpy as np
+    view = np.ctypeslib.as_array(th, shape=(M,))
+    nz = np.flatnonzero(view)
+    out["theta_nz"] = (nz, view[nz].copy())
+    if theta_at is not None:
+        out["theta_at"] = view[np.asarray(theta_at, dtype=np.int64)].copy()
+    del view
     L.lobo_destroy(h)
     return out
 

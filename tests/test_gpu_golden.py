@@ -77,18 +77,23 @@ def test_device_to_ticks_and_to_price(rlm):
         assert [G.double_bits(x) for x in outp] == [int(h, 16) for h in m["price"]], m["symbol"]
 
 
+def _unit_states(t):
+    flat = []
+    for c in t["cases"]:
+        flat += list(G.tile_vars(c))
+    return (C.c_float * len(flat))(*flat), len(t["cases"])
+
+
 def test_device_tiles(rlm, oracle):
     L = rlm.load()
     for t in G.units()["tiles"]:
-        cfg = config.from_dict(config.example_dict(**{"learning.memory_size": t["memory_size"]}))
-        n = len(t["cases"])
-        flat = []
-        for c in t["cases"]:
-            flat += [C.c_float.from_buffer_copy(C.c_uint32(u)).value for u in c["vars"]]
-        out = (C.c_int32 * (n * 9 * 96))()
-        rlm.check(L.rlm_test_tiles(C.byref(cfg), (C.c_float * len(flat))(*flat), n, out))
+        cfg = G.tile_config(t)
+        arr, n = _unit_states(t)
+        per = t["n_actions"] * 96
+        out = (C.c_int32 * (n * per))()
+        rlm.check(L.rlm_test_tiles(C.byref(cfg), arr, n, out))
         for k, c in enumerate(t["cases"]):
-            assert list(out[k * 864:(k + 1) * 864]) == c["features"], (t["memory_size"], k)
+            assert list(out[k * per:(k + 1) * per]) == c["features"], (t["memory_size"], t["n_actions"], t["n_vars"], k)
     # a larger seeded sweep against the CPU oracle (bit-exact int32 indices)
     import random
     rnd = random.Random(3)
@@ -132,3 +137,65 @@ def test_device_rolling_mean(rlm):
         for i, (a, b) in enumerate(r["mean_var"]):
             assert G.double_bits(out[2 * i]) == int(a, 16), (r["window"], i)
             assert G.double_bits(out[2 * i + 1]) == int(b, 16) or out[2 * i + 1] != out[2 * i + 1], (r["window"], i)
+
+
+# rlm_test_learner_tiles forms (include/rlm.h)
+THREE_WARP, ONE_WARP, STAGED, TRACE_GROUP0 = 0, 1, 2, 3
+
+
+def _learner_tiles(rlm, cfg, form, arr, n):
+    per = cfg.n_actions * (32 if form == TRACE_GROUP0 else 96)
+    out = (C.c_int32 * (n * per))()
+    rlm.check(rlm.load().rlm_test_learner_tiles(C.byref(cfg), form, arr, n, out))
+    return [list(out[k * per:(k + 1) * per]) for k in range(n)]
+
+
+def _forms(M):
+    return (THREE_WARP, ONE_WARP, TRACE_GROUP0) + ((STAGED,) if M <= 8192 else ())
+
+
+def _expected(form, feats, A):
+    """What a form returns for a state whose reference features are feats[a*96 + i]."""
+    if form == TRACE_GROUP0:
+        return [f for a in range(A) for f in feats[a * 96:a * 96 + 32]]
+    return feats
+
+
+def test_device_learner_tile_forms_match_the_reference(rlm):
+    """Every way the learner kernels derive a tile index -- the three-warp kernel's tile_index, the one-warp learner's
+    hash sums + ln_tile, the staged learner's 16-bit rows, and the trace passes' group-0 tiles rebuilt from the stored
+    base -- against rl::State's own features, from tables of 1 weight up to 2^31 - 1 and for 1..9 actions, 4..13
+    variables.  Above 2^30 the group-0 rebuild adds two indices below M: their sum must not wrap."""
+    for t in G.units()["tiles"]:
+        cfg = G.tile_config(t)
+        arr, n = _unit_states(t)
+        for form in _forms(t["memory_size"]):
+            got = _learner_tiles(rlm, cfg, form, arr, n)
+            for k, c in enumerate(t["cases"]):
+                assert got[k] == _expected(form, c["features"], t["n_actions"]), (form, t["memory_size"], t["n_actions"], t["n_vars"], k)
+    cfg = G.tile_config({"memory_size": 8193, "n_actions": 9, "n_vars": 8})
+    out = (C.c_int32 * 864)()
+    assert rlm.load().rlm_test_learner_tiles(C.byref(cfg), STAGED, (C.c_float * 8)(), 1, out) == abi.RLM_ERR_UNSUPPORTED
+
+
+@pytest.mark.parametrize("M", [1, 2, 3, 97, 5003, 6000, 8190, 8192, 8194, 65536, 20000000, 1 << 27, (1 << 27) + 1,
+                               (1 << 30) + 3, 3 << 29, 2 ** 31 - 1])
+def test_device_learner_tile_forms_sweep(rlm, oracle, M):
+    """Seeded states against the CPU oracle's tiles() for every form, action count and state size."""
+    import random
+    OL = oracle.lib()
+    rnd = random.Random(M)
+    n = 48
+    for A, V in ((1, 4), (5, 13), (9, 8), (2, 11)):
+        cfg = G.tile_config({"memory_size": M, "n_actions": A, "n_vars": V})
+        flat = [C.c_float(rnd.uniform(-700, 700) if rnd.random() < 0.8 else float(rnd.randint(-100, 100))).value for _ in range(n * V)]
+        arr = (C.c_float * len(flat))(*flat)
+        ref = []
+        for k in range(n):
+            out = (C.c_int32 * (A * 96))()
+            OL.lobo_tiles(C.byref(cfg), (C.c_float * V)(*flat[k * V:(k + 1) * V]), out)
+            ref.append(list(out))
+        for form in _forms(M):
+            got = _learner_tiles(rlm, cfg, form, arr, n)
+            for k in range(n):
+                assert got[k] == _expected(form, ref[k], A), (form, M, A, V, k)

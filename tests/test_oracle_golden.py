@@ -147,16 +147,20 @@ def test_rolling_mean_vectors(oracle):
 
 
 def test_tile_vectors(oracle):
-    """tiles()/hash_UNH through rl::State::populateFeatures: 9 x 96 indices per state."""
+    """tiles()/hash_UNH through rl::State::populateFeatures: n_actions x 96 indices per state, for every table size,
+    action count and state size of the unit vectors (tables of 1 weight up to 2^31 - 1)."""
     L = oracle.lib()
+    shapes = set()
     for t in G.units()["tiles"]:
-        y = config.example_dict(**{"learning.memory_size": t["memory_size"]})
-        cfg = config.from_dict(y)
+        cfg = G.tile_config(t)
         for c in t["cases"]:
-            v = (C.c_float * 8)(*[C.c_float.from_buffer_copy(C.c_uint32(u)).value for u in c["vars"]])
-            out = (C.c_int32 * (9 * 96))()
+            v = G.tile_vars(c)
+            out = (C.c_int32 * (t["n_actions"] * 96))()
             L.lobo_tiles(C.byref(cfg), v, out)
-            assert list(out) == c["features"], t["memory_size"]
+            assert list(out) == c["features"], (t["memory_size"], t["n_actions"], t["n_vars"])
+        shapes.add((t["n_actions"], t["n_vars"]))
+    assert {(a, v) for a in (1, 5, 9) for v in (4, 8, 13)} <= shapes
+    assert {1, 2, 3, 1 << 27, (1 << 27) + 1, (1 << 30) + 3, 3 << 29, 2 ** 31 - 1} <= {t["memory_size"] for t in G.units()["tiles"]}
     # SURVEY section 8c extra vector: tiles(T=32, M=20e6, {0.5,-100,-100}, int 0) -> 10174999, 12114698, ...
     t20 = [t for t in G.units()["tiles"] if t["memory_size"] == 20000000][0]["cases"][0]["features"]
     assert t20[:4] == [10174999, 12114698, 16498898, 12127300]

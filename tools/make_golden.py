@@ -70,6 +70,37 @@ F2_CASES = [
 ]
 N_F2_RECORDS = 150
 
+# The learner's configuration space beyond the defaults (9 actions, 8 or 13 variables, gamma*lambda = 0.829, tables of
+# 4096..65536): action counts whose Q sums and action hash terms sit elsewhere, feature groups of other sizes, trace lists
+# far longer than one batch of the update table (derived cap 13 408) and none at all (lambda = 0), staged tables that are
+# not powers of two, the first size past the staging limit, and tables smaller than a step's 32 tiles per group.
+# Which learner kernel a case reaches (rlm_create): staged for even M <= 8192, the one-warp learner otherwise, the
+# three-warp kernel for the R-learning agents.  150 records each, like F2_CASES.
+_VARS11 = ["pos", "spd", "mpm", "imb", "svl", "vol", "rsi", "vwap", "a_dist", "b_dist", "last_action"]
+_LONG = {"learning.gamma": 0.999, "learning.lambda": 0.99}
+CONFIG_CASES = [
+    dict(name="act1_q", algo="q_learn", M=8192, flow_seed=61, env=30, ticks=1200, over={"learning.n_actions": 1}),
+    dict(name="act2_random", algo="q_learn", M=16384, flow_seed=61, env=31, ticks=1200,
+         over={"learning.n_actions": 2, "policy.type": "random"}),
+    dict(name="act5_double_q", algo="double_q_learn", M=65536, flow_seed=63, env=32, ticks=1200, over={"learning.n_actions": 5}),
+    dict(name="act7_r_learn", algo="r_learn", M=16384, flow_seed=63, env=33, ticks=1200,
+         over={"learning.n_actions": 7, "policy.eps_init": 0.3}),
+    dict(name="vars4_sarsa", algo="sarsa", M=16384, flow_seed=65, env=34, ticks=1200,
+         over={"state.variables": ["pos", "spd", "mpm", "imb"]}),
+    dict(name="vars11_q", algo="q_learn", M=8192, flow_seed=65, env=35, ticks=1200,
+         over={"state.variables": _VARS11, "state.lookback.rsi": 6, "state.lookback.vwap": 9}),
+    dict(name="long_traces_sarsa", algo="sarsa", M=65536, flow_seed=67, env=36, ticks=1200, over=dict(_LONG)),
+    dict(name="long_traces_q", algo="q_learn", M=16384, flow_seed=67, env=37, ticks=1200, over=dict(_LONG, **{"policy.eps_init": 0.05})),
+    dict(name="lambda0_q", algo="q_learn", M=8192, flow_seed=69, env=38, ticks=1200, over={"learning.lambda": 0.0}),
+    dict(name="m6000_staged", algo="q_learn", M=6000, flow_seed=69, env=39, ticks=1200, over={}),
+    dict(name="m8190_staged_sarsa", algo="sarsa", M=8190, flow_seed=71, env=40, ticks=1200, over={}),
+    dict(name="m8194_gather", algo="q_learn", M=8194, flow_seed=71, env=41, ticks=1200, over={}),
+    dict(name="m2_staged", algo="q_learn", M=2, flow_seed=73, env=42, ticks=1200, over={}),
+    dict(name="m1_gather", algo="sarsa", M=1, flow_seed=73, env=43, ticks=1200, over={}),
+    dict(name="m3_gather", algo="q_learn", M=3, flow_seed=75, env=44, ticks=1200, over={}),
+    dict(name="m97_gather", algo="sarsa", M=97, flow_seed=75, env=45, ticks=1200, over={}),
+]
+
 # N training episodes on ONE Intraday and ONE Learner-equivalent (main.cpp:45-60, serial.cpp:72-95): the day ends
 # `open_ticks` rows after the first one, HandleTerminal(episode), LoadData of the same day again, Initialise.
 EPISODE_CASES = [
@@ -128,17 +159,7 @@ def main():
         manifest.append(dict(c, yaml=y, n_records=len(recs), summary=ref["summary"]))
         print(c["name"], len(recs), "records;", ref["summary"]["steps"], "reference steps")
     for c in F2_CASES:
-        y = config.example_dict(**{"learning.memory_size": c["M"], "learning.algorithm": c["algo"], **c["over"]})
-        y_run = json.loads(json.dumps(y))
-        y_run["debug"]["random_seed"] = y["debug"]["random_seed"] + c["env"]
-        ref = ol.run_ref(y_run, c["flow_seed"], c["env"], c["ticks"])
-        recs = ref["records"][:N_F2_RECORDS]
-        assert len(recs) == N_F2_RECORDS, (c["name"], len(recs))
-        with open(os.path.join(GOLD, "steps_%s.bin" % c["name"]), "wb") as f:
-            for r in recs:
-                f.write(bytes(r))
-        manifest.append(dict(c, yaml=y, n_records=len(recs), summary=ref["summary"]))
-        print(c["name"], len(recs), "records;", ref["summary"]["steps"], "reference steps")
+        manifest.append(short_case(c))
     for c in EPISODE_CASES:
         y = config.example_dict(**{"learning.memory_size": c["M"], "learning.algorithm": c["algo"], **c["over"]})
         y_run = json.loads(json.dumps(y))
@@ -197,9 +218,26 @@ def main():
         manifest.append(dict(c, yaml=y, backtest=True, t0_ms=t0, test=test, n_records=len(ref["records"]),
                              n_test_records=len(ref["test_records"]), summary=ref["summary"]))
         print(c["name"], len(ref["records"]), "training records;", len(ref["test_records"]), "evaluation records")
+    for c in CONFIG_CASES:
+        manifest.append(short_case(c))
     with open(os.path.join(GOLD, "manifest.json"), "w") as f:
         json.dump(manifest, f, indent=1)
     reference_checks()
+
+
+def short_case(c):
+    """The first N_F2_RECORDS records of a single-episode reference run -> steps_<name>.bin; returns the manifest entry."""
+    y = config.example_dict(**{"learning.memory_size": c["M"], "learning.algorithm": c["algo"], **c["over"]})
+    y_run = json.loads(json.dumps(y))
+    y_run["debug"]["random_seed"] = y["debug"]["random_seed"] + c["env"]
+    ref = ol.run_ref(y_run, c["flow_seed"], c["env"], c["ticks"])
+    recs = ref["records"][:N_F2_RECORDS]
+    assert len(recs) == N_F2_RECORDS, (c["name"], len(recs))
+    with open(os.path.join(GOLD, "steps_%s.bin" % c["name"]), "wb") as f:
+        for r in recs:
+            f.write(bytes(r))
+    print(c["name"], len(recs), "records;", ref["summary"]["steps"], "reference steps")
+    return dict(c, yaml=y, n_records=len(recs), summary=ref["summary"])
 
 
 def _write_digests(name, recs):
