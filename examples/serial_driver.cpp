@@ -3,9 +3,13 @@
 //
 //   g++ -std=c++17 -Iinclude examples/serial_driver.cpp -Lrl_markets_b200 -lrlm -Wl,-rpath,$PWD/rl_markets_b200 -o examples/serial_driver
 //   examples/serial_driver [--episodes N] [--algo q_learn|sarsa|double_q_learn] [--memory-size M] [--open-ticks T] [--theta out.bin]
+//                          [--md depth.csv --tas trades.csv [--symbol AAL.L] [--seed S] [--env E]]
 //
-// Prints one JSON line per episode (steps, reward, pnl) and optionally dumps theta; tests/test_gpu_facade.py checks it
-// against the fused rlm_run_ticks path.
+// Without --md/--tas every episode replays the synthetic day of the config (a short day of --open-ticks rows).  With them
+// every episode is Intraday::LoadData(symbol, md, tas) + RunEpisode on that CSV pair (tape source), like src/main.cpp's
+// loop over its file sample; --seed sets debug.random_seed and --env the env index the seeds are derived from.
+// Prints one JSON line per episode (steps, reward, pnl) and optionally dumps theta; tests/test_gpu_facade.py and
+// tests/test_gpu_tape.py check it against the fused rlm_run_ticks path.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -15,8 +19,8 @@
 
 int main(int argc, char** argv) {
   int episodes = 2, algo = RLM_ALGO_Q_LEARN, open_ticks = 400;
-  long long memory_size = 8192;
-  std::string theta_out;
+  long long memory_size = 8192, seed = -1, env_index = 0;
+  std::string theta_out, md, tas, symbol = "AAL.L";
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     auto next = [&]() { return std::string(i + 1 < argc ? argv[++i] : ""); };
@@ -24,6 +28,11 @@ int main(int argc, char** argv) {
     else if (a == "--memory-size") memory_size = atoll(next().c_str());
     else if (a == "--open-ticks") open_ticks = atoi(next().c_str());
     else if (a == "--theta") theta_out = next();
+    else if (a == "--md") md = next();
+    else if (a == "--tas") tas = next();
+    else if (a == "--symbol") symbol = next();
+    else if (a == "--seed") seed = atoll(next().c_str());
+    else if (a == "--env") env_index = atoll(next().c_str());
     else if (a == "--algo") { std::string v = next(); algo = v == "sarsa" ? RLM_ALGO_SARSA : (v == "double_q_learn" ? RLM_ALGO_DOUBLE_Q_LEARN : RLM_ALGO_Q_LEARN); }
   }
   try {
@@ -33,12 +42,17 @@ int main(int argc, char** argv) {
     c.memory_size = memory_size;
     c.flow.seed = 41;
     c.flow.t0_ms = (int32_t)(c.close_ms - 30 * 60000 - (long long)open_ticks * c.flow.dt_ms);  // a short day: it closes after open_ticks rows
-    rlm::Session session(c);
+    if (seed >= 0) c.random_seed = (uint32_t)seed;
+    c.env_index0 = env_index;
+    const bool csv = !md.empty() || !tas.empty();
+    if (csv && (md.empty() || tas.empty())) throw std::invalid_argument("--md and --tas go together");
+    rlm::Session session(c, csv ? RLM_SOURCE_TAPE : RLM_SOURCE_GENERATOR);
     rlm::environment::Intraday env(session);
     rlm::rl::Agent m(session);
     rlm::experiment::serial::Learner experiment(env);
     for (int episode = 1; episode <= episodes; ++episode) {   // train(), main.cpp:53-78
-      env.LoadData();
+      if (csv) env.LoadData(symbol, md, tas);
+      else env.LoadData();
       if (experiment.RunEpisode(&m))
         printf("{\"episode\": %d, \"steps\": %ld, \"reward\": %.17g, \"pnl\": %.17g, \"transactions\": %d}\n", episode, experiment.steps(),
                env.getEpisodeReward(), env.getEpisodePnL(), env.getTotalTransactions());

@@ -10,6 +10,8 @@
  *                         + rl::QLearn/SARSA/DoubleQLearn(policy, Config&) include/rl/agent.h:106-131
  *                         + rl::EpsilonGreedy/Greedy/Random(...)           include/rl/policy.h:31-66
  *   rlm_load_ticks        Intraday::LoadData / data::Streamer<R>           include/data/streamer.h:16-56
+ *   rlm_load_days         Intraday::LoadData for a library of days          src/environment/intraday.cpp:141-150
+ *   rlm_assign_days       ... and which day each env replays                 src/main.cpp:45-80 (sample a day per episode)
  *   rlm_reset             Intraday::Initialise                             src/environment/intraday.cpp:103-138
  *   rlm_run_ticks         experiment::serial::Learner::_step               src/experiment/serial.cpp:53-70
  *                         = Agent::action + Base::performAction + State::newState
@@ -39,7 +41,7 @@
 extern "C" {
 #endif
 
-#define RLM_ABI_VERSION 3
+#define RLM_ABI_VERSION 4
 
 typedef enum rlm_status {
   RLM_OK = 0,
@@ -68,8 +70,9 @@ enum { RLM_VAR_POS = 0, RLM_VAR_SPD, RLM_VAR_MPM, RLM_VAR_IMB, RLM_VAR_SVL, RLM_
  * "book" additionally switches the quote rule (intraday.cpp:64-71). */
 enum { RLM_TP_YAML_MIDPRICE = 0, RLM_TP_YAML_MICROPRICE = 1, RLM_TP_YAML_VWAP = 2, RLM_TP_YAML_BOOK = 3 };
 /* where ticks come from */
-enum { RLM_SOURCE_GENERATOR = 0, /* rlm_flow.h generator evaluated inside the tick kernel */
-       RLM_SOURCE_STREAM = 1 };  /* rlm_tick_msg chunks uploaded with rlm_load_ticks      */
+enum { RLM_SOURCE_GENERATOR = 0, /* rlm_flow.h generator evaluated inside the tick kernel                 */
+       RLM_SOURCE_STREAM = 1,    /* rlm_tick_msg chunks uploaded with rlm_load_ticks (tick-major, tick-aligned) */
+       RLM_SOURCE_TAPE = 2 };    /* a device-resident library of whole days (rlm_load_days), one cursor per env */
 
 #define RLM_MAX_BANDS 32 /* power of two (band search); the longest upstream table, NasdaqNordic / Oslo, has 17 bands */
 #define RLM_MAX_ACTIONS 9
@@ -168,16 +171,34 @@ int rlm_set_mode(rlm_handle h, int32_t mode);
 
 /* `environment::Intraday<> env(c)` of src/main.cpp:219: every env object is rebuilt from scratch (window sums,
  * statistics, position, book, records) while the agents keep theta, traces, generator positions and schedules.
- * `flow` (may be NULL = keep) replaces the synthetic-flow parameters, i.e. "LoadData of another day". */
+ * `flow` (may be NULL = keep) replaces the synthetic-flow parameters, i.e. "LoadData of another day" (generator source;
+ * a tape handle takes NULL only and changes days with rlm_assign_days). */
 int rlm_new_env(rlm_handle h, const rlm_flow_params* flow);
 
-/* RLM_SOURCE_STREAM: append `n_ticks` messages per env, host layout msgs[t][env] (tick-major).
+/* RLM_SOURCE_STREAM only: append `n_ticks` messages per env, host layout msgs[t][env] (tick-major).
  * The copy is issued on the handle's copy stream; the buffer must stay valid until rlm_sync. */
 int rlm_load_ticks(rlm_handle h, const rlm_tick_msg* msgs, int32_t n_ticks);
 
+/* RLM_SOURCE_TAPE: a library of whole trading days, copied to device memory once and replayed by every run call.
+ * `msgs` is the concatenation of per-day message streams exactly as rlm_ingest_csv emits them (multi-message ticks
+ * included); day d is msgs[day_offsets[d] .. day_offsets[d+1]), with day_offsets[0] = 0, non-decreasing offsets and at
+ * most 2^31 - 1 messages in all.  The call waits for the handle's work, replaces any previous library, assigns env b to
+ * day b % n_days and rewinds every env to the start of its day.  Each env reads its own day through its own cursor, one
+ * message per tick-kernel pass that ticks it (a multi-message tick takes one pass per message, as on the stream source).
+ * An env that needs a message past the end of its day stops there, inside performAction, and consumes nothing more
+ * until it is reassigned or rewound; this is not an error (rlm_env_step reports it with terminal_out = 2).
+ * rlm_reset and rlm_new_env(h, NULL) rewind every env to the start of its assigned day.
+ * Engines: tick-synchronous, round-paced and shared policy; RLM_ENGINE=F|f|p makes rlm_create fail (unsupported). */
+int rlm_load_days(rlm_handle h, const rlm_tick_msg* msgs, const int64_t* day_offsets /* [n_days + 1] */, int32_t n_days);
+/* Intraday::LoadData per env: env env0 + i replays day[i] from its first message (follow with rlm_reset, Initialise). */
+int rlm_assign_days(rlm_handle h, int32_t env0, int32_t n, const int32_t* day);
+/* messages of its assigned day each env has consumed since it was last assigned or rewound */
+int rlm_get_tape_pos(rlm_handle h, int64_t* out /* [n_envs] */);
+
 /* Advance every env by n_ticks market ticks.  Each env runs warm-up, performAction's inner NextState loop, and --
  * whenever its midprice has moved -- the complete learner step.  On return every env has consumed exactly n_ticks
- * messages and sits inside performAction's loop, whatever order the engine ran the envs' ticks in (they never interact).
+ * messages and sits inside performAction's loop, whatever order the engine ran the envs' ticks in (they never interact);
+ * on the tape source an env whose day ends earlier has consumed the rest of its day.
  * Calls shorter than 128 ticks only enqueue work (asynchronous; see rlm_sync); longer calls of independent policies on
  * up to 16 384 envs run round by round and return when the device is nearly done with them (the host follows the
  * device to learn when the last env has finished; RLM_ROUNDS=0 keeps every call asynchronous). */
@@ -235,8 +256,10 @@ int rlm_apply_dtheta(rlm_handle h);
  *     rlm_agent_update(h, delta)     state->newState(env); m->HandleTransition(...)            serial.cpp:64-67, include/rl/agent.h:62-67
  *
  * Every env advances by ONE learner step per rlm_env_step (its own K >= 1 market ticks, base.cpp:285-305); envs are
- * therefore not tick-aligned afterwards, which is why this surface needs source = generator.  actions_out[b] / the
- * action applied is -1 for an env whose episode is over.  rlm_env_step(h, actions != NULL) without a preceding rlm_act
+ * therefore not tick-aligned afterwards, which is why this surface needs source = generator or tape (not stream).
+ * actions_out[b] / the action applied is -1 for an env whose episode is over or whose tape day has run out.
+ * terminal_out[b]: 1 = the episode is over (Intraday::isTerminal), 2 = tape source: the env needed a message past the end
+ * of its day and stopped inside performAction (the reference's performAction returning false at the end of its files).  rlm_env_step(h, actions != NULL) without a preceding rlm_act
  * is the "external policy" form: no generator draw is consumed.  Independent policies only. */
 int rlm_act(rlm_handle h, int32_t* actions_out /* [n_envs] */);
 int rlm_env_step(rlm_handle h, const int32_t* actions /* [n_envs] or NULL = the agent's own */, double* reward_out /* [n_envs] or NULL */,

@@ -22,7 +22,7 @@ VAR = {"pos": 0, "spd": 1, "mpm": 2, "imb": 3, "svl": 4, "vol": 5, "rsi": 6, "vw
        "a_queue": 9, "b_dist": 10, "b_queue": 11, "last_action": 12}
 TP_YAML = {"midprice": 0, "microprice": 1, "vwap": 2, "book": 3}
 MODE_TRAIN, MODE_BACKTEST = 0, 1
-SOURCE_GENERATOR, SOURCE_STREAM = 0, 1
+SOURCE_GENERATOR, SOURCE_STREAM, SOURCE_TAPE = 0, 1, 2
 TICK_PARTIAL, TICK_TX_MORE = 1, 2  # rlm_tick_msg.flags (include/rlm_flow.h)
 
 RLM_OK = 0

@@ -63,6 +63,8 @@ struct rlm_handle_s {
   cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
   bool consumed_valid[2] = {false, false};
   int stream_ticks = 0, stream_cursor = 0;
+  // TAPE source: the day library (ptr.tape, ptr.tape_cur, ptr.tape_lo) and its day boundaries on the host
+  std::vector<int64_t> day_off;  // [n_days + 1]; empty until rlm_load_days
   void* d_gather = nullptr; void* h_gather = nullptr; size_t gather_cap = 0;  // rlm_get_reward/actions/state staging
   long long launches = 0;
   double alpha = 0, eps = 0, tau = 1.0;
@@ -364,6 +366,12 @@ static int create_impl(const rlm_config* cfg, rlm_handle_s* h) {
   }
   CK(cudaMalloc(&h->ptr.counters, 8 * 8));
   CK(cudaMemsetAsync(h->ptr.counters, 0, 8 * 8, h->stream));
+  if (cfg->source == RLM_SOURCE_TAPE) {  // per-env cursors of the day library: every env is on an empty day until rlm_load_days
+    CK(cudaMalloc(&h->ptr.tape_cur, (size_t)cfg->n_envs * sizeof(int2)));
+    CK(cudaMalloc(&h->ptr.tape_lo, (size_t)cfg->n_envs * sizeof(int)));
+    CK(cudaMemsetAsync(h->ptr.tape_cur, 0, (size_t)cfg->n_envs * sizeof(int2), h->stream));
+    CK(cudaMemsetAsync(h->ptr.tape_lo, 0, (size_t)cfg->n_envs * sizeof(int), h->stream));
+  }
   g_params_owner = nullptr;
   int rc = upload_params(h);
   if (rc != RLM_OK) return rc;
@@ -463,6 +471,11 @@ static int create_impl(const rlm_config* cfg, rlm_handle_s* h) {
       if (h->engine == 3) h->engine = 1;
     }
   }
+  if (cfg->source == RLM_SOURCE_TAPE) {
+    if (h->engine != 1) return fail(RLM_ERR_UNSUPPORTED, "the tape source runs on the tick-synchronous and round-paced engines (RLM_ENGINE=F|f|p read the stream source only)");
+    h->dyn.tape_l2 = 1;
+    if (const char* s = getenv("RLM_TAPE_PREFETCH")) h->dyn.tape_l2 = atoi(s) != 0;
+  }
   // theta is gathered 8 bytes at a time from random addresses: do not let L2 promote misses to 64/128-byte fetches
   // (device-wide, and it stays for the lifetime of the hosting process)
   cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
@@ -487,6 +500,7 @@ int rlm_destroy(rlm_handle h) {
   }
   cudaFree(h->ptr.ready); cudaFree(h->ptr.ready_count); cudaFree(h->ptr.occ); cudaFree(h->ptr.hsum);
   cudaFree(h->ptr.runctl); if (h->h_live) cudaFreeHost(h->h_live);
+  cudaFree((void*)h->ptr.tape); cudaFree(h->ptr.tape_cur); cudaFree(h->ptr.tape_lo);
   for (auto& es : h->ev_live) for (auto e : es) if (e) cudaEventDestroy(e);
   cudaFree(h->ptr.q_slots); cudaFree(h->ptr.ag_done); cudaFree(h->d_qctl);
   for (auto e : h->ev) cudaEventDestroy(e);
@@ -536,6 +550,8 @@ int rlm_set_mode(rlm_handle h, int32_t mode) {
 int rlm_new_env(rlm_handle h, const rlm_flow_params* flow) {
   API_LOCK;
   if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
+  if (flow && h->cfg.source == RLM_SOURCE_TAPE)
+    return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_new_env: a tape handle replays its day library (rlm_assign_days changes days); pass flow = NULL");
   CK(cudaSetDevice(h->cfg.device));
   if (flow) {
     CK(cudaStreamSynchronize(h->stream));  // running kernels read the old parameters from constant memory
@@ -554,7 +570,9 @@ int rlm_new_env(rlm_handle h, const rlm_flow_params* flow) {
 int rlm_load_ticks(rlm_handle h, const rlm_tick_msg* msgs, int32_t n_ticks) {
   API_LOCK;
   if (!h || !msgs || n_ticks <= 0) return fail(RLM_ERR_INVALID_ARGUMENT, "bad arguments");
-  if (h->cfg.source != RLM_SOURCE_STREAM) return fail(RLM_ERR_INVALID_ARGUMENT, "handle was created with source = generator");
+  if (h->cfg.source != RLM_SOURCE_STREAM)
+    return fail(RLM_ERR_INVALID_ARGUMENT, h->cfg.source == RLM_SOURCE_TAPE ? "rlm_load_ticks: a tape handle reads its day library (rlm_load_days)"
+                                                                           : "handle was created with source = generator");
   CK(cudaSetDevice(h->cfg.device));
   size_t n = (size_t)n_ticks * h->cfg.n_envs;
   if (!h->copy_stream) {
@@ -583,6 +601,95 @@ int rlm_load_ticks(rlm_handle h, const rlm_tick_msg* msgs, int32_t n_ticks) {
   h->ptr.stream = h->d_stream[nb];
   h->stream_ticks = n_ticks;
   h->stream_cursor = 0;
+  return RLM_OK;
+}
+
+// ---- TAPE source -------------------------------------------------------------------------------------------------
+static int tape_check(rlm_handle h) {
+  if (h->cfg.source == RLM_SOURCE_TAPE && h->day_off.empty()) return fail(RLM_ERR_INVALID_ARGUMENT, "no day library loaded (rlm_load_days)");
+  return RLM_OK;
+}
+// envs env0 .. env0+n-1 replay days day[0..n-1] from their first message (the handle's work has finished)
+static int tape_assign(rlm_handle h, int env0, int n, const int32_t* day) {
+  std::vector<int2> cur(n);
+  std::vector<int> lo(n);
+  for (int i = 0; i < n; ++i) {
+    lo[i] = (int)h->day_off[day[i]];
+    cur[i] = make_int2(lo[i], (int)h->day_off[day[i] + 1]);
+  }
+  CK(cudaMemcpy(h->ptr.tape_cur + env0, cur.data(), (size_t)n * sizeof(int2), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(h->ptr.tape_lo + env0, lo.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice));
+  return RLM_OK;
+}
+
+int rlm_load_days(rlm_handle h, const rlm_tick_msg* msgs, const int64_t* day_offsets, int32_t n_days) {
+  API_LOCK;
+  if (!h || !msgs || !day_offsets || n_days <= 0) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load_days: bad arguments");
+  if (h->cfg.source != RLM_SOURCE_TAPE) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load_days needs a handle created with source = tape");
+  if (day_offsets[0] != 0) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load_days: day_offsets[0] must be 0");
+  for (int d = 0; d < n_days; ++d)
+    if (day_offsets[d + 1] < day_offsets[d])
+      return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load_days: day_offsets must not decrease (day " + std::to_string(d) + ")");
+  const int64_t n_msgs = day_offsets[n_days];
+  if (n_msgs <= 0) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load_days: the library holds no message");
+  if (n_msgs > INT_MAX) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load_days: a day library holds at most 2^31 - 1 messages");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));  // kernels of earlier calls may still read the old library and cursors
+  {
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    const double need = (double)n_msgs * sizeof(rlm_tick_msg);
+    const double have = (double)free_b + (h->day_off.empty() ? 0.0 : (double)h->day_off.back() * sizeof(rlm_tick_msg));
+    if (need > have)
+      return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load_days: the library needs " + std::to_string((long long)(need / 1e6)) + " MB of device memory, " +
+                                                std::to_string((long long)(have / 1e6)) + " MB are free");
+  }
+  // the cached CUDA graphs hold the old library's address (DevPtrs is captured by value)
+  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
+  h->graphs.clear();
+  cudaFree((void*)h->ptr.tape);
+  h->ptr.tape = nullptr;
+  h->day_off.clear();
+  rlm_tick_msg* d_lib = nullptr;
+  CK(cudaMalloc(&d_lib, (size_t)n_msgs * sizeof(rlm_tick_msg)));
+  h->ptr.tape = d_lib;
+  CK(cudaMemcpy(d_lib, msgs, (size_t)n_msgs * sizeof(rlm_tick_msg), cudaMemcpyHostToDevice));
+  h->day_off.assign(day_offsets, day_offsets + n_days + 1);
+  std::vector<int32_t> day(h->cfg.n_envs);
+  for (int b = 0; b < h->cfg.n_envs; ++b) day[b] = b % n_days;
+  return tape_assign(h, 0, h->cfg.n_envs, day.data());
+}
+
+int rlm_assign_days(rlm_handle h, int32_t env0, int32_t n, const int32_t* day) {
+  API_LOCK;
+  if (!h || (n > 0 && !day)) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_assign_days: bad arguments");
+  if (h->cfg.source != RLM_SOURCE_TAPE) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_assign_days needs a handle created with source = tape");
+  int rc = tape_check(h);
+  if (rc) return rc;
+  if (env0 < 0 || n < 0 || (int64_t)env0 + n > h->cfg.n_envs) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_assign_days: env range out of bounds");
+  const int n_days = (int)h->day_off.size() - 1;
+  for (int i = 0; i < n; ++i)
+    if (day[i] < 0 || day[i] >= n_days)
+      return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_assign_days: day " + std::to_string(day[i]) + " of env " + std::to_string(env0 + i) +
+                                                " is not in the library (" + std::to_string(n_days) + " days)");
+  if (n == 0) return RLM_OK;
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  return tape_assign(h, env0, n, day);
+}
+
+int rlm_get_tape_pos(rlm_handle h, int64_t* out) {
+  API_LOCK;
+  if (!h || !out) return fail(RLM_ERR_INVALID_ARGUMENT, "null argument");
+  if (h->cfg.source != RLM_SOURCE_TAPE) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_get_tape_pos needs a handle created with source = tape");
+  const int B = h->cfg.n_envs;
+  std::vector<int2> cur(B);
+  std::vector<int> lo(B);
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaMemcpy(cur.data(), h->ptr.tape_cur, (size_t)B * sizeof(int2), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(lo.data(), h->ptr.tape_lo, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost));
+  for (int b = 0; b < B; ++b) out[b] = (int64_t)cur[b].x - lo[b];
   return RLM_OK;
 }
 
@@ -732,7 +839,9 @@ static int run_rounds_impl(rlm_handle h, const DynParams& d, int n_ticks) {
 }
 
 static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
-  int rc = upload_params(h);
+  int rc = tape_check(h);  // (the tape source has no upload-length check: an env whose day ends stops there)
+  if (rc) return rc;
+  rc = upload_params(h);
   if (rc) return rc;
   DynParams d = h->dyn;
   d.alpha = h->alpha; d.eps = h->eps; d.tau = h->tau; d.n_ticks = n_ticks;
@@ -1115,6 +1224,8 @@ int rlm_shared_tick_accumulate(rlm_handle h) {
   if (rc) return rc;
   DynParams d = h->dyn;
   d.alpha = h->alpha; d.eps = h->eps; d.tau = h->tau; d.n_ticks = 1;
+  rc = tape_check(h);
+  if (rc) return rc;
   if (h->cfg.source == RLM_SOURCE_STREAM && !h->in_run) {
     if (h->stream_cursor + 1 > h->stream_ticks) return fail(RLM_ERR_END_OF_DATA, "not enough ticks loaded");
     d.stream_off = h->stream_cursor; d.stream_ticks = h->stream_ticks;
@@ -1152,9 +1263,10 @@ int rlm_apply_dtheta(rlm_handle h) {
 static int split_check(rlm_handle h) {
   if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
   if (h->cfg.shared_policy) return fail(RLM_ERR_UNSUPPORTED, "the split surface drives independent policies (shared policy: rlm_shared_tick_accumulate / rlm_apply_dtheta)");
-  if (h->cfg.source != RLM_SOURCE_GENERATOR) return fail(RLM_ERR_UNSUPPORTED, "the split surface needs source = generator: envs consume different numbers of ticks per step");
+  if (h->cfg.source == RLM_SOURCE_STREAM)
+    return fail(RLM_ERR_UNSUPPORTED, "the split surface needs source = generator or tape: envs consume different numbers of ticks per step");
   if (h->dyn.backtest) return fail(RLM_ERR_UNSUPPORTED, "the split surface runs Learner::_step (train mode)");
-  return RLM_OK;
+  return tape_check(h);
 }
 static DynParams split_dyn(rlm_handle h) {
   DynParams d = h->dyn;

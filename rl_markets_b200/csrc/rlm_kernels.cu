@@ -132,6 +132,7 @@ __global__ void rlm_init_kernel(DevPtrs ptr, int mode) {
   e->ag.need_begin = 0;
   e->ag.kind = 0;
   rlm_flow_init(&e->flow, &P.flow, (uint64_t)(P.env_index0 + b));
+  if (P.source == RLM_SOURCE_TAPE) ptr.tape_cur[b].x = ptr.tape_lo[b];  // back to the first message of the env's day
 }
 
 __global__ void rlm_seed_kernel(DevPtrs ptr, unsigned random_seed) {
@@ -392,7 +393,13 @@ __global__ void rlm_step_out_kernel(DevPtrs ptr, double* reward, unsigned char* 
   if (b >= P.n_envs) return;
   const EnvHdr& e = *(const EnvHdr*)(ptr.env + (size_t)b * P.env_stride);
   if (reward) reward[b] = e.ag.last_reward;
-  if (terminal) terminal[b] = (e.phase == PH_DONE || (e.phase == PH_RUN && is_terminal(e))) ? 1 : 0;
+  if (terminal) {
+    // tape source: an env that is inside its step (not waiting for rlm_agent_update or for an action) with its day used up
+    // has stopped inside performAction -- the reference's performAction returning false at the end of its files
+    const int2 tc = P.source == RLM_SOURCE_TAPE ? ptr.tape_cur[b] : make_int2(0, 1);
+    if (e.phase != PH_DONE && !env_on_hold(e) && tc.x >= tc.y) terminal[b] = 2;
+    else terminal[b] = (e.phase == PH_DONE || (e.phase == PH_RUN && is_terminal(e))) ? 1 : 0;
+  }
   if (delta) delta[b] = e.ag.last_delta;
 }
 cudaError_t rlm_launch_act(const DevPtrs& ptr, const DynParams& D, int n_envs, int* actions, cudaStream_t st) {
@@ -569,15 +576,19 @@ __device__ __noinline__ int env_tick(EnvHdr& e, double* ring, const rlm_tick_msg
   return 0;
 }
 
-template <int THREADS>
+// TAPE: instantiation for the tape source (the other sources' code is the same as without it)
+template <int THREADS, bool TAPE>
 __global__ void __launch_bounds__(THREADS) rlm_env_kernel(DevPtrs ptr, DynParams D, int tslot, int only_begin) {
   const int b = D.env0 + blockIdx.x * THREADS + threadIdx.x;
   const int lane = threadIdx.x & 31;
   if (!only_begin) KLOG_BEGIN(0);
   int ready = -1;
   unsigned ticked = 0, errs = 0;
+  bool starved = false;  // tape source: this env needed a message past the end of its day
   if (b < (D.n_sub > 0 ? D.env0 + D.n_sub : P.n_envs)) {
     EnvHdr* g = (EnvHdr*)(ptr.env + (size_t)b * P.env_stride);
+    // tape source: the cursor comes from its own array, so its load is in flight together with the record copy below
+    const int2 tc = (TAPE && !only_begin) ? ptr.tape_cur[b] : make_int2(0, 0);
     const int ph = g->phase;
     const int nb = D.hold ? 0 : g->ag.need_begin;
     if (ph != PH_DONE && (!only_begin || nb) && !(D.hold && env_on_hold(*g))) {
@@ -602,7 +613,17 @@ __global__ void __launch_bounds__(THREADS) rlm_env_kernel(DevPtrs ptr, DynParams
       if (!only_begin && e.phase != PH_DONE) {
         rlm_tick_msg msg;
         bool have = true;
-        if (P.source == RLM_SOURCE_GENERATOR) {
+        if (TAPE) {
+          // the env's own day: message tc.x, then the cursor moves on; past the day's end the env waits inside performAction
+          if (tc.x >= tc.y) { have = false; starved = true; }
+          else {
+            const int4* src = (const int4*)(ptr.tape + tc.x);
+            int4* dst = (int4*)&msg;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) dst[i] = __ldg(src + i);
+            ptr.tape_cur[b].x = tc.x + 1;
+          }
+        } else if (P.source == RLM_SOURCE_GENERATOR) {
           flow_next_dev(&e.flow, &msg);
         } else {
           // tick-synchronous: every env consumes the same tick index.  Under a CUDA graph the call's stream pointer,
@@ -660,7 +681,7 @@ __global__ void __launch_bounds__(THREADS) rlm_env_kernel(DevPtrs ptr, DynParams
     bool still = false;
     if (b < (D.n_sub > 0 ? D.env0 + D.n_sub : P.n_envs) && ready < 0 && !only_begin) {
       const EnvHdr* g = (const EnvHdr*)(ptr.env + (size_t)b * P.env_stride);
-      still = g->phase != PH_DONE && !env_on_hold(*g);
+      still = g->phase != PH_DONE && !env_on_hold(*g) && !starved;
     }
     const unsigned rm = __ballot_sync(FULL, still);
     if (rm && lane == 0) atomicAdd(&ptr.counters[5], (unsigned long long)__popc(rm));
@@ -722,6 +743,25 @@ __device__ __forceinline__ void envw_stage_in(EnvHdr* dst_e, const EnvHdr* g, in
 #pragma unroll
   for (int k = 0; k < 4; ++k) { const int i = lane + 32 * k; if (i < n16) dst[i] = t[k]; }
 }
+// envw_stage_in on the tape source.  The env's cursor is loaded first and this lane's word of the env's next message
+// between the record's loads and their stores to shared memory: the message waits for the cursor only, never for the
+// record.  l2_next: also ask L2 for the message after it (the next launch's), one 128-byte line.
+__device__ __forceinline__ unsigned envw_stage_in_tape(EnvHdr* dst_e, const EnvHdr* g, const DevPtrs& ptr, int env, int lane, bool l2_next,
+                                                       int2& tc) {
+  tc = ptr.tape_cur[env];
+  const int4* src = (const int4*)g;
+  int4* dst = (int4*)dst_e;
+  const int n16 = (int)(envw_hdr_bytes() / 16);
+  int4 t[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { const int i = lane + 32 * k; if (i < n16) t[k] = src[i]; }
+  unsigned word = 0;
+  if (tc.x < tc.y) word = __ldg((const unsigned*)(ptr.tape + tc.x) + lane);
+  if (l2_next && lane == 0 && tc.x + 1 < tc.y) asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr.tape + tc.x + 1));
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { const int i = lane + 32 * k; if (i < n16) dst[i] = t[k]; }
+  return word;
+}
 __device__ __forceinline__ void envw_stage_out(EnvHdr* g, const EnvHdr* src_e, int lane) {
   int4* dst = (int4*)g;
   const int4* src = (const int4*)src_e;
@@ -729,16 +769,22 @@ __device__ __forceinline__ void envw_stage_out(EnvHdr* g, const EnvHdr* src_e, i
 }
 
 // One market tick of the env staged in `w`, by its warp.  stream_pos: index of this tick in the resident stream chunk.
+// Tape source: stream_pos / stream_ticks are the env's cursor and the end of its day, and tape_word is this lane's word of
+// message stream_pos, loaded by the caller ahead of the record's stage-in.
 // Returns -1, or the ready kind (0: a learner step ended -- state variables and reward are in e.ag; 1: warm-up ended).
+template <bool TAPE = false>
 __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const DevPtrs& ptr, const DynParams& D, int env, int stream_pos,
-                                         int stream_ticks, int lane, unsigned& ticked) {
+                                         int stream_ticks, int lane, unsigned& ticked, unsigned tape_word = 0) {
   EnvHdr& e = *w.e;
   rlm_tick_msg& msg = *w.msg;
   double* pushv = w.pushv;
   double* oldv = w.oldv;
   int ready = -1;
   bool have = true;
-  if (P.source == RLM_SOURCE_GENERATOR) {
+  if (TAPE) {
+    if (stream_pos >= stream_ticks) have = false;  // (callers only tick an env whose day has messages left)
+    else ((unsigned*)&msg)[lane] = tape_word;
+  } else if (P.source == RLM_SOURCE_GENERATOR) {
     flow_next_warp(&e.flow, &msg, w.r12, lane);
   } else {
     if (stream_pos >= stream_ticks) { if (lane == 0) e.err |= ERR_STREAM_UNDERRUN; have = false; }
@@ -860,6 +906,7 @@ __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const D
   return ready;
 }
 
+template <bool TAPE>
 __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr, DynParams D, int tslot, int only_begin) {
   PDL_PROLOGUE();
   extern __shared__ __align__(16) unsigned char smem[];
@@ -874,15 +921,26 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr,
   // the trailing begin-only pass touches few envs: look before staging.  A tick pass stages straight away -- one
   // memory round trip instead of two on every env's critical path -- and drops finished envs afterwards.
   if (only_begin && !g->ag.need_begin) return;
-  envw_stage_in(&e, g, lane);
+  const bool tape = TAPE && !only_begin;
+  int2 tc = make_int2(0, 0);
+  unsigned tape_word = 0;
+  if (tape) tape_word = envw_stage_in_tape(&e, g, ptr, env, lane, D.tape_l2 != 0, tc);
+  else envw_stage_in(&e, g, lane);
   __syncwarp();
   if (e.phase == PH_DONE) return;
   if (D.hold && env_on_hold(e)) return;
   int ready = -1;
   unsigned ticked = 0;
+  bool starved = false;  // tape source: this env needs a message past the end of its day
   if (e.ag.need_begin) begin_step_warp(e, ptr.mt_pol + (size_t)env * 312, D, w.flag, lane);
   if (!only_begin && e.phase != PH_DONE) {
-    if (D.ctl_stream) {  // (see rlm_env_kernel: stream pointer, offset and length of this call live in *ptr.runctl)
+    if (tape) {
+      starved = tc.x >= tc.y;
+      if (!starved) {
+        ready = envw_tick<true>(w, ring, ptr, D, env, tc.x, tc.y, lane, ticked, tape_word);
+        if (lane == 0) ptr.tape_cur[env].x = tc.x + 1;
+      }
+    } else if (D.ctl_stream) {  // (see rlm_env_kernel: stream pointer, offset and length of this call live in *ptr.runctl)
       const int4 rc4 = __ldg((const int4*)ptr.runctl);
       DevPtrs pt = ptr;
       pt.stream = (const rlm_tick_msg*)__ldg((const unsigned long long*)ptr.runctl + 2);
@@ -896,7 +954,7 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr,
   if (!only_begin) KLOG_END(0);
   if (lane == 0) {
     if (ready >= 0) ptr.ready[atomicAdd(&ptr.ready_count[tslot], 1)] = env;
-    if (D.hold && ready < 0 && e.phase != PH_DONE) atomicAdd(&ptr.counters[5], 1ull);  // still inside its step
+    if (D.hold && ready < 0 && e.phase != PH_DONE && !starved) atomicAdd(&ptr.counters[5], 1ull);  // still inside its step
     if (ticked) atomicAdd(&ptr.counters[0], 1ull);
     const unsigned errs = (unsigned)(e.err | e.ag.err);
     if (errs) atomicOr(&ptr.counters[4], (unsigned long long)errs);
@@ -909,6 +967,7 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr,
 // instead of once per market tick.  Envs never exchange anything (own book, own stream, own weights), so the order in
 // which their ticks run is not observable: per env the sequence begin_step / tick / ... / learner step is the same as
 // in the tick-synchronous engine, bit for bit.  The per-call values live in *ptr.runctl (graphs are reused across calls).
+template <bool TAPE>
 __global__ void __launch_bounds__(ENVW_WARPS * 32, 4) rlm_env_round_kernel(DevPtrs ptr, DynParams D, int tslot) {
   PDL_PROLOGUE();
   extern __shared__ __align__(16) unsigned char smem[];
@@ -928,7 +987,11 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32, 4) rlm_env_round_kernel(DevPt
   EnvHdr& e = *w.e;
   EnvHdr* g = (EnvHdr*)(ptr.env + (size_t)env * P.env_stride);
   double* ring = (double*)((unsigned char*)g + sizeof(EnvHdr));
-  envw_stage_in(&e, g, lane);
+  const bool tape = TAPE;
+  int2 tc = make_int2(0, 0);
+  unsigned tape_word = 0;
+  if (tape) tape_word = envw_stage_in_tape(&e, g, ptr, env, lane, false, tc);
+  else envw_stage_in(&e, g, lane);
   __syncwarp();
   if (e.phase == PH_DONE) return;
   int pos = e.run_id == rc.run_id ? e.run_pos : 0;
@@ -939,21 +1002,36 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32, 4) rlm_env_round_kernel(DevPt
   // next round, so that a round's tick kernel does not wait for the env with the longest run of unchanged midprices
   const int cap = D.round_cap > 0 ? D.round_cap : 0x7fffffff;
   int n_run = 0;
+  bool starved = false;  // tape source: the env's day has run out (it waits inside performAction, consuming nothing)
 #pragma unroll 1
   for (;;) {
     if (e.ag.need_begin) begin_step_warp(e, ptr.mt_pol + (size_t)env * 312, D, w.flag, lane);
     if (e.phase == PH_DONE || pos >= rc.n_ticks || n_run >= cap) break;
-    ready = envw_tick(w, ring, pt, D, env, rc.stream_off + pos, rc.stream_ticks, lane, ticked);
+    if (tape) {
+      if (tc.x >= tc.y) { starved = true; break; }
+      const unsigned word = tape_word;
+      if (tc.x + 1 < tc.y) tape_word = __ldg((const unsigned*)(ptr.tape + tc.x + 1) + lane);  // the next tick's, in flight during this one
+      ready = envw_tick<true>(w, ring, pt, D, env, tc.x, tc.y, lane, ticked, word);
+      ++tc.x;
+    } else {
+      ready = envw_tick(w, ring, pt, D, env, rc.stream_off + pos, rc.stream_ticks, lane, ticked);
+    }
     ++pos; ++n_run;
     if (ready >= 0) break;
   }
-  if (lane == 0) { e.run_id = rc.run_id; e.run_pos = pos; }
+  if (lane == 0) {
+    e.run_id = rc.run_id; e.run_pos = pos;
+    if (tape) {
+      ptr.tape_cur[env].x = tc.x;
+      if (D.tape_l2 && tc.x < tc.y) asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr.tape + tc.x));  // the next round's first
+    }
+  }
   __syncwarp();
   envw_stage_out(g, &e, lane);
   KLOG_END(0);
   if (lane == 0) {
     if (ready >= 0) ptr.ready[atomicAdd(&ptr.ready_count[tslot], 1)] = env;
-    if (ready >= 0 || (e.phase != PH_DONE && pos < rc.n_ticks)) atomicAdd(&live_count[tslot], 1);
+    if (ready >= 0 || (e.phase != PH_DONE && pos < rc.n_ticks && !starved)) atomicAdd(&live_count[tslot], 1);
     if (ticked) atomicAdd(&ptr.counters[0], (unsigned long long)ticked);
     const unsigned errs = (unsigned)(e.err | e.ag.err);
     if (errs) atomicOr(&ptr.counters[4], (unsigned long long)errs);
@@ -1998,48 +2076,53 @@ static int envw_carveout() {
 }
 cudaError_t rlm_launch_env(const DevPtrs& ptr, const DynParams& D, int n_envs, int tslot, int only_begin, int variant, cudaStream_t st) {
   if (D.n_sub > 0) n_envs = D.n_sub;  // one sub-batch
+  const bool tape = ptr.tape_cur != nullptr;  // (the cursors exist on the tape source only)
   if (variant == 1) {  // one thread per env (SIMT over envs)
     const int T = 32;
-    static bool attr1 = false;
-    if (!attr1) {
+    static bool attr1[2] = {false, false};
+    if (!attr1[tape]) {
       // this kernel uses no shared memory at all; its per-thread record copy lives in local memory, i.e. in L1 (RLM_ENVT_CARVEOUT)
       int c = RLM_ENVT_CARVEOUT_DEFAULT;
       if (const char* e = getenv("RLM_ENVT_CARVEOUT")) { const int v = atoi(e); if (v >= 0 && v <= 100) c = v; }
-      cudaFuncSetAttribute(rlm_env_kernel<T>, cudaFuncAttributePreferredSharedMemoryCarveout, c);
-      attr1 = true;
+      cudaFuncSetAttribute(tape ? rlm_env_kernel<T, true> : rlm_env_kernel<T, false>, cudaFuncAttributePreferredSharedMemoryCarveout, c);
+      attr1[tape] = true;
     }
-    rlm_env_kernel<T><<<(n_envs + T - 1) / T, T, 0, st>>>(ptr, D, tslot, only_begin);
+    if (tape) rlm_env_kernel<T, true><<<(n_envs + T - 1) / T, T, 0, st>>>(ptr, D, tslot, only_begin);
+    else rlm_env_kernel<T, false><<<(n_envs + T - 1) / T, T, 0, st>>>(ptr, D, tslot, only_begin);
     return cudaGetLastError();
   }
   const int W = envw_warps_per_cta();
   const size_t smem = (size_t)W * envw_warp_bytes();
-  static bool attr = false;
-  if (!attr) {
+  auto kern = tape ? rlm_env_kernel_w<true> : rlm_env_kernel_w<false>;
+  static bool attr[2] = {false, false};
+  if (!attr[tape]) {
     if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(rlm_env_kernel_w, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
     }
     // the same L1/shared split as the learner kernel: CTAs of the two kernels (different sub-batches, different streams)
     // can then share an SM instead of waiting for it to drain and be reconfigured
-    cudaFuncSetAttribute(rlm_env_kernel_w, cudaFuncAttributePreferredSharedMemoryCarveout, envw_carveout());
-    attr = true;
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, envw_carveout());
+    attr[tape] = true;
   }
-  return launch_pdl(rlm_env_kernel_w, (n_envs + W - 1) / W, W * 32, smem, st, ptr, D, tslot, only_begin);
+  return launch_pdl(kern, (n_envs + W - 1) / W, W * 32, smem, st, ptr, D, tslot, only_begin);
 }
 
 cudaError_t rlm_launch_env_round(const DevPtrs& ptr, const DynParams& D, int n_envs, int tslot, cudaStream_t st) {
   const int W = envw_warps_per_cta();
   const size_t smem = (size_t)W * envw_warp_bytes();
-  static bool attr = false;
-  if (!attr) {
+  const bool tape = ptr.tape_cur != nullptr;
+  auto kern = tape ? rlm_env_round_kernel<true> : rlm_env_round_kernel<false>;
+  static bool attr[2] = {false, false};
+  if (!attr[tape]) {
     if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(rlm_env_round_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
     }
-    cudaFuncSetAttribute(rlm_env_round_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, envw_carveout());
-    attr = true;
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, envw_carveout());
+    attr[tape] = true;
   }
-  return launch_pdl(rlm_env_round_kernel, (n_envs + W - 1) / W, W * 32, smem, st, ptr, D, tslot);
+  return launch_pdl(kern, (n_envs + W - 1) / W, W * 32, smem, st, ptr, D, tslot);
 }
 cudaError_t rlm_launch_runctl(const DevPtrs& ptr, const RunCtl& v, cudaStream_t st) {
   rlm_runctl_kernel<<<1, 1, 0, st>>>(ptr.runctl, v);

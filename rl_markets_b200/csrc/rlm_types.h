@@ -155,6 +155,7 @@ struct DynParams {  // changes between launches (HandleTerminal / GoGreedy)
   int round_cap;      // round-paced engine: most ticks an env runs in one round (RLM_ROUND_CAP; 0 = up to its step end)
   int ctl_stream;     // tick-synchronous engine under a CUDA graph, STREAM source: stream pointer / offset / length come from *DevPtrs::runctl
   int hold;           // split surface (rlm_env_step): envs whose step has ended, or whose next action is not applied yet, do not tick
+  int tape_l2;        // tape source: the warp-per-env tick kernels ask L2 for each env's next message (RLM_TAPE_PREFETCH, default 1)
 };
 
 // ready counters: [RLM_MAX_SUB][RLM_READY_CAP] ints, followed by as many live counters (round-paced engine)
@@ -192,4 +193,9 @@ struct DevPtrs {
   int q_size;                    // power of two >= n_envs
   int pad;
   RunCtl* runctl;                // round-paced engine: the current run call
+  // tape source (rlm_load_days): the day library and each env's read position in it.  The cursor lives here and not in
+  // the env record so that a tick kernel can form the message address without waiting for the record's stage-in.
+  const rlm_tick_msg* tape;      // [n_msgs] concatenated days
+  int2* tape_cur;                // [n_envs] {next message, end of the env's day} (absolute message indices)
+  int* tape_lo;                  // [n_envs] first message of the env's day (rlm_reset / rlm_new_env rewind to it)
 };

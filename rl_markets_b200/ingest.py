@@ -61,6 +61,23 @@ def csv_pair_to_ticks(md_path, tas_path):
     return lib.ingest_csv(md_path, tas_path)
 
 
+def day_library(samples):
+    """The (symbol, md csv, tas csv) tuples of file_sample / sample_window -> (msgs, offsets) for BatchedMarket.load_days:
+    every pair through rlm_ingest_csv, the message streams one after the other, offsets[d] = first message of day d and
+    offsets[-1] = the total."""
+    import ctypes as C
+    from . import abi
+    days = [lib.ingest_csv(md, tas) for _symbol, md, tas in samples]
+    offsets = [0]
+    for _msgs, n, _ticks in days:
+        offsets.append(offsets[-1] + n)
+    out = (abi.TickMsg * max(offsets[-1], 1))()
+    size = C.sizeof(abi.TickMsg)
+    for (msgs, n, _ticks), off in zip(days, offsets):
+        C.memmove(C.addressof(out) + off * size, msgs, n * size)
+    return out, offsets
+
+
 def load_day(market, md_path, tas_path):
     """Intraday::LoadData (src/environment/intraday.cpp:141-150) for every env of a STREAM-source handle: the same day for
     all of them.  Returns the number of message slots to pass to run_ticks."""

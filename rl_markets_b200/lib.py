@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get("RLM_LIB_PATH") or os.path.join(_HERE, "librlm.so")  #
 
 EXPORTS = [
     "rlm_last_error", "rlm_abi_version", "rlm_config_default", "rlm_create", "rlm_destroy", "rlm_reset", "rlm_set_mode", "rlm_new_env",
-    "rlm_load_ticks", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
+    "rlm_load_ticks", "rlm_load_days", "rlm_assign_days", "rlm_get_tape_pos", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
     "rlm_get_reward", "rlm_get_actions", "rlm_get_rho", "rlm_get_occupancy", "rlm_copy_theta", "rlm_handle_terminal", "rlm_go_greedy", "rlm_read_theta",
     "rlm_write_theta", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
     "rlm_set_stream", "rlm_set_profiling", "rlm_get_kernel_times", "rlm_act", "rlm_env_step", "rlm_agent_update", "rlm_ingest_csv",
@@ -51,6 +51,9 @@ def load():
     L.rlm_set_mode.argtypes = [C.c_void_p, C.c_int32]
     L.rlm_new_env.argtypes = [C.c_void_p, P(abi.FlowParams)]
     L.rlm_load_ticks.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+    L.rlm_load_days.argtypes = [C.c_void_p, C.c_void_p, P(C.c_int64), C.c_int32]
+    L.rlm_assign_days.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_int32)]
+    L.rlm_get_tape_pos.argtypes = [C.c_void_p, P(C.c_int64)]
     L.rlm_run_ticks.argtypes = [C.c_void_p, C.c_int32]
     L.rlm_sync.argtypes = [C.c_void_p]
     L.rlm_get_counters.argtypes = [C.c_void_p, P(abi.Counters)]
@@ -154,6 +157,25 @@ class BatchedMarket:
         addr = msgs if isinstance(msgs, int) else C.addressof(msgs)
         check(self.L.rlm_load_ticks(self.h, addr, n_ticks))
 
+    def load_days(self, msgs, offsets):
+        """Tape source: upload a library of days once (rlm_load_days).  msgs: ctypes array (or address) of TickMsg, the days
+        one after the other; offsets: n_days + 1 message offsets (day d = msgs[offsets[d]:offsets[d + 1]]).  Env b replays
+        day b % n_days from its start."""
+        offs = (C.c_int64 * len(offsets))(*offsets)
+        addr = msgs if isinstance(msgs, int) else C.addressof(msgs)
+        check(self.L.rlm_load_days(self.h, addr, offs, len(offsets) - 1))
+
+    def assign_days(self, days, env0=0):
+        """Tape source: env env0 + i replays day days[i] from its first message (Intraday::LoadData per env)."""
+        n = len(days)
+        check(self.L.rlm_assign_days(self.h, env0, n, (C.c_int32 * max(n, 1))(*days)))
+
+    def tape_pos(self):
+        """Tape source: messages of its day each env has consumed since it was assigned or rewound."""
+        out = (C.c_int64 * self.cfg.n_envs)()
+        check(self.L.rlm_get_tape_pos(self.h, out))
+        return list(out)
+
     def run_ticks(self, n):
         check(self.L.rlm_run_ticks(self.h, n))
 
@@ -233,7 +255,8 @@ class BatchedMarket:
         return out
 
     def env_step(self, actions=None):
-        """Base::performAction + getReward: one learner step's worth of ticks per env.  Returns (rewards, terminal)."""
+        """Base::performAction + getReward: one learner step's worth of ticks per env.  Returns (rewards, terminal):
+        terminal[b] is 1 when env b's episode is over, 2 when its tape day ran out inside performAction (tape source)."""
         n = self.cfg.n_envs
         rew, term = (C.c_double * n)(), (C.c_uint8 * n)()
         check(self.L.rlm_env_step(self.h, actions, rew, term))
