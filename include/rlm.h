@@ -287,7 +287,10 @@ int rlm_flow_generate(const rlm_flow_params* p, int64_t env_index, int64_t first
                       rlm_tick_msg* out);
 
 /* ---- unit-level device entry points for the golden vectors of the reference's tests ---- */
-/* Market::ToTicks / ToPrice (test/test_Market.cpp) evaluated ON THE DEVICE */
+/* Market::ToTicks / ToPrice (test/test_Market.cpp) evaluated ON THE DEVICE; out = -1 (-1.0) where the reference throws.
+ * rlm_test_to_ticks converts px[0..n) in order in one thread and carries one band hint from each price to the next,
+ * as an env does (starting from band 0), so an order that jumps between bands exercises hint misses; the hint never
+ * changes a result. */
 int rlm_test_to_ticks(const rlm_config* cfg, const double* px, int32_t n, int32_t* out);
 int rlm_test_to_price(const rlm_config* cfg, const int32_t* ticks, int32_t n, double* out);
 /* tiles() (src/rl/tiles.cpp:31-75) for n states of n_vars floats, all actions: out[n][n_actions][96] */

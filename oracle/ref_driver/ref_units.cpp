@@ -13,7 +13,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <random>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
@@ -288,6 +290,76 @@ int main() {
              stp + 1 < nsteps ? "," : "");
     }
     printf("  ]}%s\n", sc < 11 ? "," : "");
+  }
+  printf("],\n");
+
+  // ---------------------------------------------------------------- ToTicks / ToPrice around every band boundary
+  // For each band start b below the top band: b and its neighbouring doubles, the half-tick points below it, a dozen
+  // prices in (b - ts_above/2, b - ts_below/2) where ToTicks' loop enters band b with ub < b and `int += double`
+  // truncates one tick away, the first ticks above it, float-widened grid prices (what the book holds) on both sides;
+  // then seeded prices in every band, half of them on a half-tick (where the quotient meets an integer, so a division
+  // rounded differently changes the result).  Nothing reaches the top band or the half tick below it (SURVEY A16).
+  // ToPrice at every tts_ key and its neighbours; null = the reference throws (negative price / tick count).
+  // A generator of its own keeps the vectors of the other sections as they were.
+  printf("\"market_sweep\": [\n");
+  {
+    uint64_t s = 4242;
+    auto next = [&s]() -> uint32_t { s = s * 6364136223846793005ull + 1442695040888963407ull; return (uint32_t)(s >> 33); };
+    auto unit = [&next]() { return ((double)next() + 0.5) / 4294967296.0; };
+    struct Peek : market::Market { using market::Market::pts_; using market::Market::tts_; };
+    for (int si = 0; si < n_syms; ++si) {
+      market::Market* m = market::Market::make_market(syms[si][0], syms[si][1]);
+      const map<double, double>& pts = m->*(&Peek::pts_);
+      const map<int, double>& tts = m->*(&Peek::tts_);
+      vector<double> bx, bt;
+      for (auto& kv : pts) { bx.push_back(kv.first); bt.push_back(kv.second); }
+      const int nb = (int)bx.size();
+      const double top = bx[nb - 1] - bt[nb - 1];  // every price stays below this
+      vector<double> px = {-nextafter(0.0, 1.0), -bt[0]};
+      auto add = [&px, top](double p) { if (p < top) px.push_back(p); };
+      for (int k = 0; k <= nb - 2; ++k) {
+        const double b = bx[k], ta = bt[k];
+        add(b); add(nextafter(b, 1e300)); add(b + ta / 2.0); add(b + ta); add((double)(float)(b + ta));
+        if (k == 0) continue;
+        const double tb = bt[k - 1], eps = 1.0 / 1048576.0;
+        add(nextafter(b, -1e300));
+        for (double f : {1.0, 0.5 + eps, 0.5, 0.5 - eps}) add(b - tb * f);
+        const double lo = b - ta / 2.0, hi = b - tb / 2.0;
+        if (lo < hi) {
+          add(nextafter(lo, 1e300)); add(nextafter(hi, -1e300));
+          for (int j = 0; j < 12; ++j) add(lo + (hi - lo) * (j + 0.5) / 12.0);
+        }
+        for (int j = 0; j < 4; ++j) { add((double)(float)(b + j * ta)); add((double)(float)(b - (j + 1) * tb)); }
+      }
+      for (int i = 0; i < 300; ++i) {
+        const int k = (int)(next() % (unsigned)(nb - 1));
+        const double span = bx[k + 1] - bx[k];
+        double p;
+        if (i & 1) p = bx[k] + ((double)(next() % (unsigned)(span / bt[k])) + 0.5) * bt[k];
+        else p = bx[k] + unit() * span;
+        if (i % 4 == 3) p = (double)(float)p;
+        add(p);
+      }
+      printf("  {\"symbol\": \"%s.%s\", \"px\": [", syms[si][0], syms[si][1]);
+      for (size_t i = 0; i < px.size(); ++i) { printf("%s", i ? ", " : ""); p_d(px[i]); }
+      printf("], \"ticks\": [");
+      for (size_t i = 0; i < px.size(); ++i) {
+        printf("%s", i ? ", " : "");
+        try { printf("%d", m->ToTicks(px[i])); } catch (const std::invalid_argument&) { printf("null"); }
+      }
+      vector<int> tq;
+      const int last_key = tts.rbegin()->first;
+      for (auto& kv : tts) { tq.push_back(kv.first - 1); tq.push_back(kv.first); if (kv.first < last_key) tq.push_back(kv.first + 1); }
+      printf("], \"tq\": [");
+      for (size_t i = 0; i < tq.size(); ++i) printf("%s%d", i ? ", " : "", tq[i]);
+      printf("], \"price\": [");
+      for (size_t i = 0; i < tq.size(); ++i) {
+        printf("%s", i ? ", " : "");
+        try { p_d(m->ToPrice(tq[i])); } catch (const std::invalid_argument&) { printf("null"); }
+      }
+      printf("]}%s\n", si + 1 < n_syms ? "," : "");
+      delete m;
+    }
   }
   printf("]\n}\n");
   return 0;

@@ -428,15 +428,6 @@ static int create_impl(const rlm_config* cfg, rlm_handle_s* h) {
   }
   // persistent engine: queue + flags
   {
-    int q = 1;
-    while (q < cfg->n_envs) q <<= 1;
-    h->ptr.q_size = q;
-    CK(cudaMalloc(&h->ptr.q_slots, (size_t)q * 4));
-    CK(cudaMemsetAsync(h->ptr.q_slots, 0xFF, (size_t)q * 4, h->stream));
-    CK(cudaMalloc(&h->ptr.ag_done, (size_t)cfg->n_envs * 4));
-    CK(cudaMemsetAsync(h->ptr.ag_done, 0, (size_t)cfg->n_envs * 4, h->stream));
-    CK(cudaMalloc(&h->d_qctl, 4 * 4));
-    h->ptr.q_head = h->d_qctl; h->ptr.q_tail = h->d_qctl + 1; h->ptr.env_warps_done = h->d_qctl + 2; h->ptr.q_done = (int*)(h->d_qctl + 3);
     // agent CTAs must all be resident; leave at least a quarter of the slots to env CTAs
     const int resident = rlm_run_max_resident_ctas(p.scratch_bytes, h->n_sms);
     const int n_env_ctas = (cfg->n_envs + 127) / 128;
@@ -444,6 +435,18 @@ static int create_impl(const rlm_config* cfg, rlm_handle_s* h) {
     int cap = resident - std::min(n_env_ctas, std::max(resident / 4, 1));
     h->n_agent_ctas = std::max(1, std::min(want, cap));
     if (const char* s = getenv("RLM_AGENT_CTAS")) { int v = atoi(s); if (v > 0 && v < resident) h->n_agent_ctas = v; }
+    // Every agent warp holds one ticket while it waits, and ticket t waits on slot t % q_size: the ring needs a slot per
+    // waiting warp as well as per env.  With fewer slots (1 or 2 envs: 4 agent warps) several warps spin on one slot and
+    // more than one can take the same push -- two learner steps on one env at once.
+    int q = 1;
+    while (q < cfg->n_envs || q < h->n_agent_ctas * RLM_RUN_WARPS) q <<= 1;
+    h->ptr.q_size = q;
+    CK(cudaMalloc(&h->ptr.q_slots, (size_t)q * 4));
+    CK(cudaMemsetAsync(h->ptr.q_slots, 0xFF, (size_t)q * 4, h->stream));
+    CK(cudaMalloc(&h->ptr.ag_done, (size_t)cfg->n_envs * 4));
+    CK(cudaMemsetAsync(h->ptr.ag_done, 0, (size_t)cfg->n_envs * 4, h->stream));
+    CK(cudaMalloc(&h->d_qctl, 4 * 4));
+    h->ptr.q_head = h->d_qctl; h->ptr.q_tail = h->d_qctl + 1; h->ptr.env_warps_done = h->d_qctl + 2; h->ptr.q_done = (int*)(h->d_qctl + 3);
     // engines: 's' tick-synchronous (two launches per tick), 'F' fused persistent round-2 kernel, 'f' round-1 fused kernel,
     // 'p' persistent queue
     if (const char* s = getenv("RLM_ENGINE")) h->engine = (s[0] == 'p') ? 0 : ((s[0] == 'f') ? 2 : ((s[0] == 'F') ? 3 : 1));

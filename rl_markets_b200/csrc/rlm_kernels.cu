@@ -1910,8 +1910,8 @@ cudaError_t rlm_launch_fused(const DevPtrs& ptr, const DynParams& D, int n_envs,
 //                             its warp keep ticking.  Envs advance at their own pace (their results do
 //                             not depend on the schedule: all state is per env).
 // Agent CTAs come first in the grid, so they are resident before any env CTA can wait on them.
-#define RUN_THREADS 128
-#define RUN_WARPS (RUN_THREADS / 32)
+#define RUN_WARPS RLM_RUN_WARPS
+#define RUN_THREADS (RUN_WARPS * 32)
 
 __device__ __forceinline__ void copy_ag_from_global(AgentD& dst, const AgentD* src) {
   const int4* s = (const int4*)src;
@@ -2168,10 +2168,16 @@ cudaError_t rlm_launch_clear_traces(const DevPtrs& ptr, int n_envs, cudaStream_t
 
 // ---------------------------------------------------------------------------------------------
 // unit-level device entry points (golden vectors of the reference's tests)
+// one thread, in order, carrying one band hint from price to price the way an env carries EnvHdr::tk_band (zeroed at
+// creation), so that a sequence that jumps between bands exercises both the hinted and the searched band look-up
 __global__ void k_test_to_ticks(const double* px, int n, int* out) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  int err = 0;
-  if (i < n) { int t = to_ticks(px[i], &err); out[i] = err ? -1 : t; }
+  if (threadIdx.x || blockIdx.x) return;
+  int hint = 0;
+  for (int i = 0; i < n; ++i) {
+    int err = 0;
+    const int t = to_ticks(px[i], &err, &hint);
+    out[i] = err ? -1 : t;
+  }
 }
 __global__ void k_test_to_price(const int* ticks, int n, double* out) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2245,7 +2251,7 @@ __global__ void k_test_rolling_mean(const double* vals, int n, double* out, doub
   }
 }
 
-cudaError_t rlm_launch_test_to_ticks(const double* px, int n, int* out) { k_test_to_ticks<<<(n + 127) / 128, 128>>>(px, n, out); return cudaGetLastError(); }
+cudaError_t rlm_launch_test_to_ticks(const double* px, int n, int* out) { k_test_to_ticks<<<1, 32>>>(px, n, out); return cudaGetLastError(); }
 cudaError_t rlm_launch_test_to_price(const int* t, int n, double* out) { k_test_to_price<<<(n + 127) / 128, 128>>>(t, n, out); return cudaGetLastError(); }
 cudaError_t rlm_launch_test_tiles(const float* vars, int n, int* out) { k_test_tiles<<<(n + 3) / 4, 128>>>(vars, n, out); return cudaGetLastError(); }
 cudaError_t rlm_launch_test_learner_tiles(int form, const float* vars, int n, int* out) {

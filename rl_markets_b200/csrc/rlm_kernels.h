@@ -19,6 +19,7 @@ cudaError_t rlm_launch_apply_dtheta(double* theta, double* dtheta, long long n, 
 size_t rlm_fused_smem_bytes(int is_double);
 cudaError_t rlm_launch_fused(const DevPtrs& ptr, const DynParams& D, int n_envs, int is_double, cudaStream_t st);
 cudaError_t rlm_launch_run(const DevPtrs& ptr, const DynParams& D, int n_envs, int scratch_bytes, int n_agent_ctas, cudaStream_t st);
+#define RLM_RUN_WARPS 4  // warps per CTA of the persistent engine (rlm_run_kernel)
 int rlm_run_max_resident_ctas(int scratch_bytes, int n_sms);
 cudaError_t rlm_launch_act(const DevPtrs& ptr, const DynParams& D, int n_envs, int* actions, cudaStream_t st);
 cudaError_t rlm_launch_apply(const DevPtrs& ptr, const DynParams& D, int n_envs, const int* actions, cudaStream_t st);

@@ -3,7 +3,9 @@ import ctypes as C
 import hashlib
 import json
 import os
+import random
 import struct
+import sys
 
 from rl_markets_b200 import abi, config
 
@@ -17,12 +19,31 @@ def _all_cases():
 
 def manifest():
     """Single-episode training cases."""
-    return [c for c in _all_cases() if not c.get("backtest") and not c.get("multi_episode") and not c.get("ingest")]
+    return [c for c in _all_cases() if not c.get("backtest") and not c.get("multi_episode") and not c.get("ingest")
+            and not c.get("venue_day")]
 
 
 def ingest_manifest():
     """Reference runs on CSV pairs with real-data irregularities (tools/messy_csv.py); the pair is committed beside them."""
     return [c for c in _all_cases() if c.get("ingest")]
+
+
+def venue_manifest():
+    """Reference runs on whole trading days of other venues, whose best bid crosses a band boundary of the venue's tick
+    table (tools/venue_csv.py); the CSV pair is written again by venue_day(), records are stored as digests."""
+    return [c for c in _all_cases() if c.get("venue_day")]
+
+
+def venue_day(case, d, seed=None):
+    """Write the CSV pair of a venue case (or another day of the same writer, `seed`) into directory d -> (md, tas)."""
+    tools = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools")
+    if tools not in sys.path:
+        sys.path.insert(0, tools)
+    import venue_csv
+    md, tas = os.path.join(d, "v_md_1.csv"), os.path.join(d, "v_tas_1.csv")
+    venue_csv.write_day(md, tas, case["ticker"], case["boundary"], case["day_seed"] if seed is None else seed,
+                        thin=case.get("thin", False))
+    return md, tas
 
 
 def ingest_paths(case):
@@ -86,6 +107,18 @@ def tile_config(entry):
 def tile_vars(case):
     """The state of a units.json tile case as a ctypes float array (stored as bit patterns)."""
     return (C.c_float * len(case["vars"]))(*[C.c_float.from_buffer_copy(C.c_uint32(u)).value for u in case["vars"]])
+
+
+def sweep_sequence(entry):
+    """A units.json market_sweep entry as (prices, expected ticks, None where the reference throws), in the order the
+    conversions are fed: ascending, so each band is entered once from below, then a seeded shuffle of the same points,
+    so a conversion carrying the previous one's band hint usually finds it stale."""
+    px = [hex_to_double(h) for h in entry["px"]]
+    order = sorted(range(len(px)), key=lambda i: px[i])
+    shuffled = list(range(len(px)))
+    random.Random(entry["symbol"]).shuffle(shuffled)
+    idx = order + shuffled
+    return [px[i] for i in idx], [entry["ticks"][i] for i in idx]
 
 
 def hex_to_double(h):

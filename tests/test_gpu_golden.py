@@ -75,6 +75,21 @@ def test_device_to_ticks_and_to_price(rlm):
         outp = (C.c_double * nt)()
         rlm.check(L.rlm_test_to_price(C.byref(cfg), (C.c_int32 * nt)(*m["tq"]), nt, outp))
         assert [G.double_bits(x) for x in outp] == [int(h, 16) for h in m["price"]], m["symbol"]
+    # every band boundary of every venue table, fed through one band hint in an order that keeps it stale (the market
+    # vectors above also pass through the hint, in their own order); -1 / -1.0 where the reference throws
+    for m in G.units()["market_sweep"]:
+        cfg = config.from_dict(config.example_dict(), ticker=m["symbol"])
+        px, ticks = G.sweep_sequence(m)
+        n = len(px)
+        out = (C.c_int32 * n)()
+        rlm.check(L.rlm_test_to_ticks(C.byref(cfg), (C.c_double * n)(*px), n, out))
+        bad = [(p, t, o) for p, t, o in zip(px, ticks, out) if o != (-1 if t is None else t)]
+        assert not bad, (m["symbol"], len(bad), bad[:5])
+        nt = len(m["tq"])
+        outp = (C.c_double * nt)()
+        rlm.check(L.rlm_test_to_price(C.byref(cfg), (C.c_int32 * nt)(*m["tq"]), nt, outp))
+        want = [G.double_bits(-1.0) if h is None else int(h, 16) for h in m["price"]]
+        assert [G.double_bits(x) for x in outp] == want, m["symbol"]
 
 
 def _unit_states(t):

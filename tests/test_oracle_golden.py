@@ -128,6 +128,27 @@ def test_market_vectors(oracle):
             assert G.double_bits(L.lobo_to_price(C.byref(cfg), t)) == int(h, 16), (m["symbol"], t)
 
 
+def test_market_band_sweep(oracle):
+    """ToTicks / ToPrice around every band boundary of every venue table (units.json market_sweep): both sides of each
+    band start, the window below it where the reference's loop steps into the next band and subtracts a tick, tick sizes
+    that are not powers of two, and every tts_ key.  The oracle throws where the reference does, so those points are
+    left to the device test, which reports them as -1."""
+    L = oracle.lib()
+    sweep = G.units()["market_sweep"]
+    assert len(sweep) == 16
+    for m in sweep:
+        cfg = config.from_dict(config.example_dict(), ticker=m["symbol"])
+        px, ticks = G.sweep_sequence(m)
+        assert ticks.count(None) == 4, m["symbol"]  # the two negative prices, in both passes
+        got = [L.lobo_to_ticks(C.byref(cfg), p) for p, t in zip(px, ticks) if t is not None]
+        assert got == [t for t in ticks if t is not None], m["symbol"]
+        for t, h in zip(m["tq"], m["price"]):
+            if h is None:
+                assert t < 0, (m["symbol"], t)
+                continue
+            assert G.double_bits(L.lobo_to_price(C.byref(cfg), t)) == int(h, 16), (m["symbol"], t)
+
+
 def test_rolling_mean_vectors(oracle):
     """test/test_Accumulators.cpp: RollingMean<double> mean/var on sliding windows."""
     L = oracle.lib()

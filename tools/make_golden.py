@@ -7,6 +7,7 @@ machines without the reference can check against them).
   tests/golden/units.json          reference unit-level vectors (oracle/_ref/ref_units)
   tests/golden/steps_<name>.bin    first N rlm_step_record of a reference run (oracle/_ref/ref_driver)
   tests/golden/bt_*_{profit_log,test_stats}.csv   the reference's own evaluation logs for the backtest cases
+  tests/golden/digests_venue_*.bin per-record digests of the reference on whole venue days (tools/venue_csv.py)
   tests/golden/manifest.json       the configs that produced them
 """
 import ctypes as C
@@ -132,6 +133,43 @@ BACKTEST_CASES = [
 ]
 
 
+# Whole trading days of other venues (tools/venue_csv.py): the best bid crosses one band boundary of the venue's tick
+# table many times, and the day ends at the venue's own close.  One case per distinct tick table, each with its own agent
+# and quote rule; target-price quoting puts quotes inside the window below a boundary where ToTicks subtracts a tick.
+# X.S is a thin book (1..20 lots per level, order size 10, positions within +-20): market orders walk past the depth the
+# book shows, cancellations meet volume queued behind an order, and an order's level vanishes.  The CSV pairs are not
+# committed: the tests write them again and check them against the sha256 stored here.
+VENUE_CASES = [
+    dict(name="venue_aal_l", ticker="AAL.L", boundary=5000.0, day_seed=101, algo="q_learn", M=8192, env=50,
+         over={"market.target_price.type": "book", "state.variables": _ALL_VARS, "state.lookback.rsi": 10,
+               "state.lookback.vwap": 20}),
+    dict(name="venue_baes_l", ticker="BAES.L", boundary=500.0, day_seed=102, algo="sarsa", M=8192, env=51, over={}),
+    dict(name="venue_x_pa", ticker="X.PA", boundary=50.0, day_seed=103, algo="double_q_learn", M=8192, env=52,
+         over={"market.target_price.type": "microprice", "market.target_price.lookback": 5}),
+    dict(name="venue_x_st", ticker="X.ST", boundary=5000.0, day_seed=104, algo="r_learn", M=8192, env=53,
+         over={"policy.eps_init": 0.3}),
+    dict(name="venue_x_mi", ticker="X.MI", boundary=2.0, day_seed=105, algo="q_learn", M=5003, env=54,
+         over={"policy.type": "boltzmann", "policy.tau_init": 0.05, "policy.tau_floor": 0.01, "policy.tau_T": 10}),
+    dict(name="venue_x_vi", ticker="X.VI", boundary=10.0, day_seed=106, algo="sarsa", M=4096, env=55,
+         over={"market.target_price.type": "vwap", "reward.measure": "mm_linear", "reward.pos_weight": 0.5}),
+    dict(name="venue_x_i", ticker="X.I", boundary=10.0, day_seed=107, algo="double_q_learn", M=8192, env=56, over={}),
+    dict(name="venue_x_co", ticker="X.CO", boundary=0.5, day_seed=108, algo="q_learn", M=8192, env=57,
+         over={"reward.measure": "pnl"}),
+    dict(name="venue_x_s", ticker="X.S", boundary=1000.0, day_seed=109, algo="q_learn", M=4096, env=58, thin=True,
+         over={"market.order_size": 10, "market.pos_ub": 20, "market.pos_lb": -20, "policy.eps_init": 0.5}),
+]
+
+
+def venue_yaml(c):
+    return config.example_dict(**{"learning.memory_size": c["M"], "learning.algorithm": c["algo"], "data.symbols": [c["ticker"]],
+                                  **c["over"]})
+
+
+def file_sha256(path):
+    import hashlib
+    return hashlib.sha256(open(path, "rb").read()).hexdigest()
+
+
 def day_t0(cfg, open_ticks, dt_ms=250):
     """t0 such that the market closes (venue close - 30 min, market.cpp:67-70) `open_ticks` rows after the first one."""
     return int(cfg.close_ms) - 30 * 60000 - open_ticks * dt_ms
@@ -220,9 +258,39 @@ def main():
         print(c["name"], len(ref["records"]), "training records;", len(ref["test_records"]), "evaluation records")
     for c in CONFIG_CASES:
         manifest.append(short_case(c))
+    import golden_util
+    import test_venue_days
+    for c in VENUE_CASES:
+        y = venue_yaml(c)
+        with tempfile.TemporaryDirectory() as d:
+            md, tas = golden_util.venue_day(c, d)
+            raw, summary = test_venue_days.reference_on_day(ol, c, y, md, tas, d)
+            sha = dict(md_sha256=file_sha256(md), tas_sha256=file_sha256(tas))
+        recs = list((abi.StepRecord * (len(raw) // C.sizeof(abi.StepRecord))).from_buffer_copy(raw))
+        assert summary["terminal"] == 1 and len(recs) == summary["steps"]
+        _write_digests(c["name"], recs)  # whole days: 8-byte digests per record instead of ~220 KB of records each
+        manifest.append(dict(c, yaml=y, venue_day=True, n_records=len(recs), summary=summary, **sha))
+    _keep_wall_clock(manifest)
     with open(os.path.join(GOLD, "manifest.json"), "w") as f:
         json.dump(manifest, f, indent=1)
     reference_checks()
+
+
+def _keep_wall_clock(manifest):
+    """The reference's run time is in the summaries it printed; an entry whose outputs did not change keeps the stored
+    time, so that regenerating leaves manifest.json as it was."""
+    path = os.path.join(GOLD, "manifest.json")
+    if not os.path.exists(path):
+        return
+    old = {c["name"]: c for c in json.load(open(path))}
+    clock = ("seconds", "steps_per_s")
+    for c in manifest:
+        o = old.get(c["name"])
+        if o is None or "summary" not in o:
+            continue
+        same = {k: v for k, v in o["summary"].items() if k not in clock} == {k: v for k, v in c["summary"].items() if k not in clock}
+        if same and json.dumps(dict(o, summary=None)) == json.dumps(dict(json.loads(json.dumps(c)), summary=None)):
+            c["summary"] = o["summary"]
 
 
 def short_case(c):
