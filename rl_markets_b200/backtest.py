@@ -40,7 +40,8 @@ def test_stats_rows(records, market_sells, market_buys):
 
 def write_logs(market, out_dir, env=0, date=20100104):
     """Write profit_log.csv / test_stats.csv / theta.bin for recorded env `env` of a handle in backtest mode
-    (every step of the episode must be recorded: cfg.record_cap >= steps)."""
+    (every step of the episode must be recorded: cfg.record_cap >= steps).  theta.bin is the policy env `env` ran under:
+    its own, or the handle's one policy when cfg.shared_policy is set."""
     os.makedirs(out_dir, exist_ok=True)
     recs, _keep = market.records(env)
     paths = {k: os.path.join(out_dir, v) for k, v in
@@ -54,5 +55,5 @@ def write_logs(market, out_dir, env=0, date=20100104):
         for k, v in test_stats_rows(recs, st.market_sells, st.market_buys):
             f.write("%s,%d\n" % (k, v))
     with open(paths["theta"], "wb") as f:
-        f.write(bytes(market.theta(env)))
+        f.write(bytes(market.theta(0 if market.cfg.shared_policy else env)))
     return paths

@@ -263,16 +263,18 @@ static int derive(rlm_handle_s* h) {
 
 static cudaError_t launch_agent_on(rlm_handle_s* h, const DevPtrs& ptr, const DynParams& d, int tslot, int stage, cudaStream_t st) {
   const int n = d.n_sub > 0 ? d.n_sub : h->cfg.n_envs;  // worst case: every env of the (sub-)batch is ready
+  // backtest mode: the greedy evaluation step is the same for every algorithm and for independent and shared policies
+  if (d.backtest) return rlm_launch_eval(ptr, d, n, h->hp.is_double, tslot, h->n_sms, st);
   // Q-learning / SARSA / Double-Q training: the one-warp-per-env learner (rlm_learn.cuh).  The R-learning agents' third
-  // evaluation and the backtest step stay on the three-warp kernel's EXTRAS instantiation.
-  if (h->agent_variant == 4 && !d.backtest && h->cfg.algorithm < RLM_ALGO_R_LEARN) {
+  // evaluation stays on the three-warp kernel's EXTRAS instantiation.
+  if (h->agent_variant == 4 && h->cfg.algorithm < RLM_ALGO_R_LEARN) {
     // small per-env tables: the whole table is staged in shared memory by one bulk copy per step (rlm_learn_staged_kernel)
     if (h->staged && stage == 0) return rlm_launch_learn_staged(ptr, d, n, h->cfg.memory_size, tslot, h->n_sms, st);
     // steps a launch usually finds: ~29 % of the envs per tick, ~57 % per round of at most three ticks
     return rlm_launch_learn(ptr, d, n, h->hp.is_double, tslot, h->n_sms, stage, h->in_rounds ? (n * 3 + 4) / 5 : (n * 3 + 9) / 10, st);
   }
   if (h->agent_variant >= 3) {
-    const int full = (d.backtest || h->cfg.algorithm >= RLM_ALGO_R_LEARN) ? 1 : 0;
+    const int full = (h->cfg.algorithm >= RLM_ALGO_R_LEARN) ? 1 : 0;
     return rlm_launch_agent3(ptr, d, n, h->hp.is_double, h->hp.occ_smem_words, tslot, h->n_sms, stage, full, st);
   }
   return rlm_launch_agent(ptr, d, n, h->hp.scratch_bytes, tslot, h->n_sms, stage, st);
@@ -545,7 +547,7 @@ int rlm_set_mode(rlm_handle h, int32_t mode) {
   if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
   if (mode != RLM_MODE_TRAIN && mode != RLM_MODE_BACKTEST) return fail(RLM_ERR_INVALID_ARGUMENT, "unknown mode");
   if (mode == RLM_MODE_BACKTEST && h->engine != 1 && h->engine != 3) return fail(RLM_ERR_UNSUPPORTED, "backtest mode runs on the tick-synchronous engine only");
-  if (mode == RLM_MODE_BACKTEST && h->cfg.shared_policy) return fail(RLM_ERR_UNSUPPORTED, "backtest mode with shared_policy is not built");
+  if (h->dyn.backtest != mode) h->graph_warm = false;  // (the other mode's kernel: its first call launches directly, see run_ticks_impl)
   h->dyn.backtest = mode;
   return RLM_OK;
 }
@@ -855,8 +857,9 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
     d.stream_ticks = h->stream_ticks;
     h->stream_cursor += n_ticks;
   }
-  if (h->cfg.shared_policy) {
-    // single-GPU shared policy: every tick = accumulate, apply (no all-reduce needed)
+  if (h->cfg.shared_policy && !d.backtest) {
+    // single-GPU shared policy: every tick = accumulate, apply (no all-reduce needed).  Evaluation (backtest mode) never
+    // writes theta, so it needs neither stage: it takes the tick-synchronous path below with every env reading policy 0.
     const DynParams keep = h->dyn;
     h->in_run = true;
     for (int t = 0; t < n_ticks; ++t) {
@@ -1215,6 +1218,8 @@ int rlm_device_ptrs(rlm_handle h, void** theta, void** dtheta, int64_t* n_double
   if (n_doubles) *n_doubles = h->cfg.shared_policy ? (int64_t)(h->hp.is_double ? 2 : 1) * h->cfg.memory_size : (int64_t)h->n_policies * h->cfg.memory_size;
   return RLM_OK;
 }
+static const char* const k_eval_no_collective =
+    "backtest mode: evaluation never writes theta, so it needs no collective -- call rlm_run_ticks (every rank evaluates its own envs)";
 // Shared policy, phase A of one tick: env tick + learner steps evaluated under theta_t, updates
 // accumulated into dtheta.  The caller all-reduces dtheta (rlm_device_ptrs) across ranks when the policy
 // spans GPUs, then calls rlm_apply_dtheta.
@@ -1222,6 +1227,7 @@ int rlm_shared_tick_accumulate(rlm_handle h) {
   API_LOCK;
   if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
   if (!h->cfg.shared_policy) return fail(RLM_ERR_INVALID_ARGUMENT, "handle was not created with shared_policy");
+  if (h->dyn.backtest) return fail(RLM_ERR_INVALID_ARGUMENT, k_eval_no_collective);
   CK(cudaSetDevice(h->cfg.device));
   int rc = upload_params(h);
   if (rc) return rc;
@@ -1248,10 +1254,11 @@ int rlm_apply_dtheta(rlm_handle h) {
   API_LOCK;
   if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
   if (!h->cfg.shared_policy) return fail(RLM_ERR_INVALID_ARGUMENT, "handle was not created with shared_policy");
+  if (h->dyn.backtest) return fail(RLM_ERR_INVALID_ARGUMENT, k_eval_no_collective);
   CK(cudaSetDevice(h->cfg.device));
   int rc = upload_params(h);
   if (rc) return rc;
-  const long long n = (long long)(h->hp.is_double ? 2 : 1) * h->cfg.memory_size;
+  const long long n =(long long)(h->hp.is_double ? 2 : 1) * h->cfg.memory_size;
   CK(rlm_launch_apply_dtheta(h->ptr.theta, h->ptr.dtheta, h->cfg.memory_size, h->n_sms, h->stream));
   if (h->hp.is_double) CK(rlm_launch_apply_dtheta(h->ptr.theta_b, h->ptr.dtheta + h->cfg.memory_size, h->cfg.memory_size, h->n_sms, h->stream));
   (void)n;

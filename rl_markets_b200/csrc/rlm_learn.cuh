@@ -593,6 +593,119 @@ cudaError_t rlm_launch_learn(const DevPtrs& ptr, const DynParams& D, int n_envs,
 }
 
 // ---------------------------------------------------------------------------------------------
+// Greedy evaluation step (backtest mode; experiment::serial::Backtester::_step, serial.cpp:121-137): the front third of
+// ln_step.  The state of the NEXT action is the env's current one and nothing is learned, so a step is: stage the agent
+// block, hash the to-state, gather, exact-order sums, Q -> q_from.  theta, dtheta and the trace lists are only read, so
+// any number of envs may share one table (shared_policy: every env reads policy 0) with no reduction of any kind -- each
+// env is exactly one reference process that loaded that table.  The step is the same for all six algorithms: the
+// R-learning agents' action selection needs Q_A / Q_B only, never rho.
+// Per step: [AgentD 704][V], 7.6 KB (Double-Q 14.5 KB) -- no tile table, no update table, no trace access.
+#define EV_WARPS 4  // steps (warps) per CTA
+template <bool DBL> struct EvCfg { static constexpr int min_ctas = DBL ? 3 : 4; };  // 12 / 16 steps per SM (168 / 128 registers)
+__host__ __device__ inline size_t ev_warp_bytes(int is_double) { return (size_t)LN_AG_BYTES + ln_v_bytes(is_double); }
+// 16-byte chunk c of the agent block holds a field an evaluation step writes: Q_A/Q_B(from, .), last_delta, n_steps,
+// from_vars | from_base0 | null_from .. ep_step.  The generator states, rho, prev_vars and to_vars are not written back.
+__device__ __forceinline__ bool ev_chunk_written(int c) {
+  const int lo = 16 * c, hi = lo + 16;
+  return lo < (int)offsetof(AgentD, to_vars) || (hi > (int)offsetof(AgentD, from_base0) && lo < (int)offsetof(AgentD, crand_r)) ||
+         (hi > (int)offsetof(AgentD, null_from) && lo < (int)offsetof(AgentD, err));
+}
+
+template <bool DBL>
+__global__ void __launch_bounds__(EV_WARPS * 32, EvCfg<DBL>::min_ctas) rlm_eval_kernel(DevPtrs ptr, DynParams D, int tslot) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned char* wsm = smem + (size_t)warp * ev_warp_bytes(DBL ? 1 : 0);
+  AgentD& ag = *(AgentD*)wsm;
+  double* V = (double*)(wsm + LN_AG_BYTES);
+  // (see rlm_learn_kernel: the hashing table, pulled into L1 under the ready-count and agent-block round trips)
+  for (int i = threadIdx.x; i < 64; i += EV_WARPS * 32) asm volatile("prefetch.global.L1 [%0];" ::"l"(rlm_rndseq_table + i * 32));
+  const int n_ready = ptr.ready_count[tslot];
+  unsigned long long steps_done = 0;
+  if (n_ready > (int)blockIdx.x) KLOG_BEGIN(1);
+  constexpr int N16 = (int)(AG_BYTES / 16);
+  static_assert(N16 > 32 && N16 <= 64, "two 16-byte loads per lane cover the agent block");
+  const int C = gridDim.x;  // ready env k -> warp (k / C) of CTA (k % C): a short list spreads over all SMs
+#pragma unroll 1
+  for (int idx = warp * C + blockIdx.x; idx < n_ready; idx += EV_WARPS * C) {
+    const int env = ptr.ready[idx];
+    EnvHdr* g = (EnvHdr*)(ptr.env + (size_t)env * P.env_stride);
+    {
+      const int4* src = (const int4*)&g->ag;
+      int4* dst = (int4*)&ag;
+      const int4 t0 = __ldcg(src + lane);
+      int4 t1 = make_int4(0, 0, 0, 0);
+      if (lane + 32 < N16) t1 = __ldcg(src + lane + 32);
+      dst[lane] = t0;
+      if (lane + 32 < N16) dst[lane + 32] = t1;
+    }
+    __syncwarp();
+    const int kind = ag.kind;  // 0: a step ended, 1: Intraday::Initialise ended (the first action of the day)
+    if (kind == 0 || kind == 1) {
+      const size_t pol = P.shared_policy ? 0 : (size_t)env;
+      const double* theta_a = ptr.theta + pol * (size_t)P.memory_size;
+      const LnSums h = ln_hash(rlm_rndseq_table, ag.to_vars, false, lane);
+      {
+        double va[3 * RLM_MAX_ACTIONS];
+        ln_gather_issue<0, 27>(theta_a, h, va);
+        if (DBL) {  // both tables' 54 gathers in flight together
+          double vb[3 * RLM_MAX_ACTIONS];
+          ln_gather_issue<0, 27>(ptr.theta_b + pol * (size_t)P.memory_size, h, vb);
+          ln_gather_store<0, 27>(vb, lane, V + RLM_MAX_ACTIONS * LN_VROW);
+        }
+        ln_gather_store<0, 27>(va, lane, V);
+      }
+      __syncwarp();
+      const double q = ln_sums(V, DBL, lane);
+      if (kind == 0) {  // the step that just ended, recorded with the state its action was chosen from
+        if (lane == 0) ag.last_delta = 0.0;
+        __syncwarp();
+        if (env < P.record_envs) emit_record_ool(ptr, g, env, ag, theta_a, ag.from_vars, lane);
+        __syncwarp();
+        steps_done++;
+      }
+      ln_store_q<DBL>(ag, q, lane);
+      if (lane < RLM_N_STATE_MAX + 3) ag.from_vars[lane] = ag.to_vars[lane];
+      ag.from_base0[lane] = mod_m(h.s[0]);
+      if (lane == 0) {
+        ag.null_from = 0; ag.need_begin = 1;
+        if (kind == 0) { ag.n_steps++; ag.ep_step++; } else ag.kind = 2;
+      }
+      __syncwarp();
+      int4* dst = (int4*)&g->ag;
+      const int4* src = (const int4*)&ag;
+      if (ev_chunk_written(lane)) __stcg(dst + lane, src[lane]);
+      if (lane + 32 < N16 && ev_chunk_written(lane + 32)) __stcg(dst + lane + 32, src[lane + 32]);
+    }
+    __syncwarp();  // (every lane is done with the block before the next env is staged over it)
+  }
+  if (steps_done) KLOG_END(1);
+  if (lane == 0 && steps_done) atomicAdd(&ptr.counters[1], steps_done);
+}
+
+cudaError_t rlm_launch_eval(const DevPtrs& ptr, const DynParams& D, int n_envs, int is_double, int tslot, int n_sms, cudaStream_t st) {
+  const int k = is_double ? 1 : 0;
+  const size_t smem = EV_WARPS * ev_warp_bytes(is_double);
+  static int per_sm[2] = {0, 0};  // resident CTAs per SM
+  if (!per_sm[k]) {
+    cudaError_t e = is_double ? cudaFuncSetAttribute(rlm_eval_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                              : cudaFuncSetAttribute(rlm_eval_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    if (is_double) cudaFuncSetAttribute(rlm_eval_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, RLM_SMEM_CARVEOUT);
+    else cudaFuncSetAttribute(rlm_eval_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, RLM_SMEM_CARVEOUT);
+    int n = 0;
+    e = is_double ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, rlm_eval_kernel<true>, EV_WARPS * 32, smem)
+                  : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, rlm_eval_kernel<false>, EV_WARPS * 32, smem);
+    per_sm[k] = (e == cudaSuccess && n > 0) ? n : 1;
+  }
+  // one resident wave at most; the grid-stride loop takes the rest
+  const int grid = std::min((n_envs + EV_WARPS - 1) / EV_WARPS, n_sms * per_sm[k]);
+  if (is_double) rlm_eval_kernel<true><<<grid, EV_WARPS * 32, smem, st>>>(ptr, D, tslot);
+  else rlm_eval_kernel<false><<<grid, EV_WARPS * 32, smem, st>>>(ptr, D, tslot);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------
 // Fused persistent engine (the default for independent-policy training): ONE launch per rlm_run_ticks call, one warp
 // per env for all `n_ticks` ticks.  The env record stays in shared memory for the whole launch; the warp runs the market
 // tick (envw_tick) and, whenever its env's midprice has moved, the learner step (ln_step) and the next action selection

@@ -239,6 +239,15 @@ class BatchedMarket:
         check(self.L.rlm_read_theta(self.h, policy, table, out, n))
         return out
 
+    def write_theta(self, values, policy=0, table=0):
+        """Load one weight table (memory_size doubles; table 1 = Q_B of the double agents) into policy `policy` -- policy 0 is
+        the only one of a shared_policy handle: load a trained policy there, go_greedy(), set_mode(MODE_BACKTEST) and every
+        env evaluates it on its own day."""
+        n = self.cfg.memory_size
+        buf = values if isinstance(values, C.Array) and values._type_ is C.c_double else (C.c_double * n).from_buffer_copy(bytes(values))
+        assert len(buf) == n, (len(buf), n)
+        check(self.L.rlm_write_theta(self.h, policy, table, buf, n))
+
     def set_profiling(self, on):
         check(self.L.rlm_set_profiling(self.h, 1 if on else 0))
 
