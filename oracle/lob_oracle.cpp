@@ -661,6 +661,7 @@ struct lobo_env {
   std::vector<double> theta, theta_b;
   // shared-policy batch (SURVEY section 8e): theta lives in the batch object, updates go to dtheta
   std::vector<double>*sh_a = nullptr, *sh_b = nullptr, *sh_da = nullptr, *sh_db = nullptr;
+  std::vector<lobo_contrib>* contrib_log = nullptr;  // the batch's contribution log while it is on (lobo_batch_log)
   std::vector<double>& THA() { return sh_a ? *sh_a : theta; }
   std::vector<double>& THB() { return sh_b ? *sh_b : theta_b; }
   bool is_double() const { return c.algorithm == RLM_ALGO_DOUBLE_Q_LEARN || c.algorithm == RLM_ALGO_DOUBLE_R_LEARN; }
@@ -722,7 +723,7 @@ struct lobo_env {
   // position all start from scratch) driven by the SAME agent (theta, traces, generators, schedules)
   void new_env() {
     lobo_env* f = new lobo_env();
-    f->sh_a = sh_a; f->sh_b = sh_b; f->sh_da = sh_da; f->sh_db = sh_db;
+    f->sh_a = sh_a; f->sh_b = sh_b; f->sh_da = sh_da; f->sh_db = sh_db; f->contrib_log = contrib_log;
     f->init(&c, env_index);
     f->theta.swap(theta); f->theta_b.swap(theta_b);
     f->traces = traces;
@@ -1002,6 +1003,16 @@ struct lobo_env {
   double maxQ(State& s) { return getQ(s, argmaxQ(s)); }  // :171-174
   void updateQ_tab(std::vector<double>& th, double update) {  // :137-142 / :232-237
     double scaled_update = update / c.n_tilings;
+    if (contrib_log) {  // shared-policy batch with the log on: the same additions, each one also recorded
+      const int32_t table = (&th == sh_db) ? 1 : 0;
+      for (int k = 0; k < traces.n; ++k) {
+        int f = traces.nonzero[k];
+        double v = scaled_update * traces.eligibility[f];
+        th[f] += v;
+        contrib_log->push_back({table, f, v});
+      }
+      return;
+    }
     for (int k = 0; k < traces.n; ++k) { int f = traces.nonzero[k]; th[f] += scaled_update * traces.eligibility[f]; }
   }
   // policies (src/rl/policy.cpp)
@@ -1404,6 +1415,7 @@ struct lobo_batch {
   std::vector<lobo_env*> envs;
   std::vector<double> th_a, th_b, d_a, d_b;
   std::vector<int> pending;
+  std::vector<lobo_contrib> log;  // this tick's dtheta additions, in the order they were made (lobo_batch_log)
 };
 
 lobo_batch* lobo_batch_create(const rlm_config* cfg) {
@@ -1428,6 +1440,7 @@ void lobo_batch_destroy(lobo_batch* b) { for (auto* e : b->envs) delete e; delet
 // phase A of one tick for every env: msgs[env]; step records (if recs) are written at recs[env*rec_cap + count[env]]
 void lobo_batch_accumulate(lobo_batch* b, const rlm_tick_msg* msgs, rlm_step_record* recs, int32_t* rec_count, int32_t rec_cap) {
   b->pending.clear();
+  b->log.clear();
   for (size_t i = 0; i < b->envs.size(); ++i) {
     rlm_step_record* r = nullptr;
     if (recs && rec_count[i] < rec_cap) r = &recs[i * (size_t)rec_cap + rec_count[i]];
@@ -1443,7 +1456,16 @@ void lobo_batch_apply(lobo_batch* b) {
   for (int i : b->pending) b->envs[i]->begin_step();
   b->pending.clear();
 }
+void lobo_batch_log(lobo_batch* b, int on) {
+  b->log.clear();
+  for (auto* e : b->envs) e->contrib_log = on ? &b->log : nullptr;
+}
+const lobo_contrib* lobo_batch_log_entries(lobo_batch* b, int64_t* n) {
+  *n = (int64_t)b->log.size();
+  return b->log.data();
+}
 int64_t lobo_batch_steps(lobo_batch* b) { int64_t s = 0; for (auto* e : b->envs) s += e->total_steps; return s; }
+int64_t lobo_batch_sum_traces(lobo_batch* b) { int64_t s = 0; for (auto* e : b->envs) s += e->sum_traces; return s; }
 void lobo_batch_stats(lobo_batch* b, int32_t env, rlm_env_stats* out) { lobo_stats(b->envs[env], out); }
 
 int32_t lobo_to_ticks(const rlm_config* cfg, double px) { Venue v{}; v.init(cfg); return v.ToTicks(px); }

@@ -62,7 +62,15 @@ void lobo_batch_accumulate(lobo_batch* b, const rlm_tick_msg* msgs /* [n_envs] *
 double* lobo_batch_dtheta(lobo_batch* b, int table);
 double* lobo_batch_theta(lobo_batch* b, int table);
 void lobo_batch_apply(lobo_batch* b);
+/* Contribution log: with it on, every addition a batch env makes into dtheta during lobo_batch_accumulate is also
+ * recorded as (table, feature, value), value being exactly the double added (scaled_update * eligibility[f]).  The
+ * log holds the last accumulate's entries in the order they were added; switching it on or off clears it.  With the
+ * log off nothing is recorded and every number is what it was without it. */
+typedef struct lobo_contrib { int32_t table; int32_t feature; double value; } lobo_contrib;
+void lobo_batch_log(lobo_batch* b, int on);
+const lobo_contrib* lobo_batch_log_entries(lobo_batch* b, int64_t* n);
 int64_t lobo_batch_steps(lobo_batch* b);
+int64_t lobo_batch_sum_traces(lobo_batch* b);  /* trace entries summed over every step of every env (rlm_counters) */
 void lobo_batch_stats(lobo_batch* b, int32_t env, rlm_env_stats* out);
 
 /* ---- unit-level entry points (golden vectors) ---- */
