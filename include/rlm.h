@@ -12,6 +12,7 @@
  *   rlm_load_ticks        Intraday::LoadData / data::Streamer<R>           include/data/streamer.h:16-56
  *   rlm_load_days         Intraday::LoadData for a library of days          src/environment/intraday.cpp:141-150
  *   rlm_assign_days       ... and which day each env replays                 src/main.cpp:45-80 (sample a day per episode)
+ *   rlm_set_day_markets   ... under the market of the day's ticker          src/environment/intraday.cpp:141-150
  *   rlm_reset             Intraday::Initialise                             src/environment/intraday.cpp:103-138
  *   rlm_run_ticks         experiment::serial::Learner::_step               src/experiment/serial.cpp:53-70
  *                         = Agent::action + Base::performAction + State::newState
@@ -198,6 +199,25 @@ int rlm_load_days(rlm_handle h, const rlm_tick_msg* msgs, const int64_t* day_off
 int rlm_assign_days(rlm_handle h, int32_t env0, int32_t n, const int32_t* day);
 /* messages of its assigned day each env has consumed since it was last assigned or rewound */
 int rlm_get_tape_pos(rlm_handle h, int64_t* out /* [n_envs] */);
+
+/* One venue's Market (src/market/market.cpp:11-38,67-70): the same fields and rules as rlm_config's venue block. */
+typedef struct rlm_market {
+  int32_t n_bands; int32_t pad;
+  double band_px[RLM_MAX_BANDS];
+  double band_ts[RLM_MAX_BANDS];
+  int64_t open_ms, close_ms;
+} rlm_market;
+/* RLM_SOURCE_TAPE: day d of the loaded library runs under markets[day_market[d]] (Intraday::LoadData building the
+ * ticker's market, src/environment/intraday.cpp:141-150) -- its tick table decides ToTicks / ToPrice, its hours the
+ * warm-up start and the terminal step.  n_days must equal the library's day count.
+ * - Tape handles only, with a library loaded.  The call waits for the handle's work and, like rlm_load_days, rewinds
+ *   every env to the start of its assigned day: follow it with rlm_reset.
+ * - An env's market follows its day, through rlm_load_days' b % n_days assignment and through rlm_assign_days.
+ * - rlm_load_days replaces the library and drops the day markets: every day runs under the config's market again.
+ * - Every market gets the checks rlm_create applies to the config's (1..RLM_MAX_BANDS bands, ascending band_px,
+ *   positive band_ts) and every index must lie in [0, n_markets); otherwise RLM_ERR_INVALID_ARGUMENT, nothing changed.
+ * - Training and backtest, independent and shared policies and the split surface all read the env's market. */
+int rlm_set_day_markets(rlm_handle h, const rlm_market* markets, int32_t n_markets, const int32_t* day_market, int32_t n_days);
 
 /* Advance every env by n_ticks market ticks.  Each env runs warm-up, performAction's inner NextState loop, and --
  * whenever its midprice has moved -- the complete learner step.  On return every env has consumed exactly n_ticks

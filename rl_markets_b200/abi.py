@@ -178,6 +178,18 @@ class Config(C.Structure):
     ]
 
 
+class Market(C.Structure):
+    """rlm_market: one venue's tick table and trading hours (rlm_set_day_markets)."""
+    _fields_ = [
+        ("n_bands", C.c_int32),
+        ("pad", C.c_int32),
+        ("band_px", C.c_double * RLM_MAX_BANDS),
+        ("band_ts", C.c_double * RLM_MAX_BANDS),
+        ("open_ms", C.c_int64),
+        ("close_ms", C.c_int64),
+    ]
+
+
 class Counters(C.Structure):
     _fields_ = [
         ("ticks", C.c_int64),

@@ -69,6 +69,40 @@ def venue_table(ticker):
     raise ValueError('[Market] Unknown exchange venue "%s".' % venue)
 
 
+def _fill_venue(dst, ticker):
+    bands, mo, mc = venue_table(ticker)
+    dst.n_bands = len(bands)
+    for i, (px, ts) in enumerate(bands):
+        dst.band_px[i] = px
+        dst.band_ts[i] = ts
+    dst.open_ms, dst.close_ms = mo, mc
+    return dst
+
+
+def market(ticker):
+    """abi.Market of 'SYMBOL.VENUE' (Market::make_market, src/market/market.cpp:40-61): the tick table and trading hours
+    rlm_create takes from the config's first symbol, for rlm_set_day_markets.  Raises as venue_table does."""
+    return _fill_venue(abi.Market(), ticker)
+
+
+def config_market(cfg):
+    """abi.Market of a handle's config (its venue block)."""
+    m = abi.Market()
+    m.n_bands = cfg.n_bands
+    for i in range(abi.RLM_MAX_BANDS):
+        m.band_px[i] = cfg.band_px[i]
+        m.band_ts[i] = cfg.band_ts[i]
+    m.open_ms, m.close_ms = cfg.open_ms, cfg.close_ms
+    return m
+
+
+def same_market(a, b):
+    """The same tick table and trading hours (unused band slots ignored)."""
+    n = a.n_bands
+    return (n == b.n_bands and a.open_ms == b.open_ms and a.close_ms == b.close_ms
+            and all(a.band_px[i] == b.band_px[i] and a.band_ts[i] == b.band_ts[i] for i in range(n)))
+
+
 def _get(d, path, default=None, required=False):
     cur = d
     for k in path:
@@ -172,12 +206,7 @@ def from_dict(y, n_envs=1, ticker=None, device=0, env_index0=0, shared_policy=Fa
     if ticker is None:
         syms = _get(y, ("data", "symbols"), ["AAL.L"])
         ticker = syms[0]
-    bands, mo, mc = venue_table(ticker)
-    c.n_bands = len(bands)
-    for i, (px, ts) in enumerate(bands):
-        c.band_px[i] = px
-        c.band_ts[i] = ts
-    c.open_ms, c.close_ms = mo, mc
+    _fill_venue(c, ticker)
     # debug
     seed = _get(y, ("debug", "random_seed"))
     if seed is None:

@@ -92,7 +92,13 @@ extern "C" int rlm_debug_klog(unsigned long long* out, int reset) {
 #define KLOG_END(kind) do { } while (0)
 #endif
 
-cudaError_t rlm_upload_params(const DevParams* p) { return cudaMemcpyToSymbol(P, p, sizeof(DevParams)); }
+// whether the uploaded block has day markets on: the launchers then pick the tick kernels' MKT instantiations
+static bool g_day_markets = false;
+cudaError_t rlm_upload_params(const DevParams* p, const DevMarkets* m) {
+  g_day_markets = m->markets != nullptr;
+  const cudaError_t e = cudaMemcpyToSymbol(P, p, sizeof(DevParams));
+  return e != cudaSuccess ? e : cudaMemcpyToSymbol(PM, m, sizeof(DevMarkets));
+}
 
 // ---------------------------------------------------------------------------------------------
 // init: Intraday ctor/Initialise state + RNG seeding, one thread per env.
@@ -250,21 +256,27 @@ __device__ __noinline__ void fill_record(rlm_step_record* r, const EnvHdr& e, co
 //   begin_select  Agent::action(*last_state) -- or the end of the episode (isTerminal, ClearInventory serial.cpp:31)
 //   begin_apply   Base::performAction(action) up to its do-while (DoAction, CheckOrders, UpdateStats, first reward term)
 // Needs ag.q_from / qb_from.  begin_select returns the action, or -1 when the episode is over.
-__device__ __noinline__ int begin_select(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D) {
-  if (is_terminal(e)) {
+template <class... M>
+__device__ __forceinline__ int begin_select_in(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D, M... mk) {
+  if (is_terminal(e, mk...)) {
     clear_inventory(e);  // Runner::RunEpisode, serial.cpp:31
     e.phase = PH_DONE;
     return -1;
   }
   return policy_action(e.ag, e.ag.q_from, e.ag.qb_from, mt_pol, D);
 }
-__device__ __noinline__ void begin_apply(EnvHdr& e, int a) {
+__device__ __noinline__ int begin_select(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D) { return begin_select_in(e, mt_pol, D); }
+__device__ __noinline__ int begin_select(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D, EnvMarket mk) {
+  return begin_select_in(e, mt_pol, D, mk);
+}
+template <class... M>
+__device__ __forceinline__ void begin_apply_in(EnvHdr& e, int a, M... mk) {
   e.ag.cur_action = a;
   e.last_action = a;
   e.lo_vol_step = 0;
   e.pnl_step = 0.0;
   e.momentum_pnl_step = 0.0;
-  do_action(e, a);
+  do_action(e, a, mk...);
   check_orders(e);
   update_stats(e);
   e.agg_r = get_reward(e);
@@ -272,21 +284,25 @@ __device__ __noinline__ void begin_apply(EnvHdr& e, int a) {
   e.agg_mpm = 0.0;
   e.ag.kind = 3;  // inside performAction's loop (0 / 1 = the step / the warm-up has ended and waits for the learner)
 }
-__device__ __forceinline__ bool begin_step(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D) {
-  if (e.ag.kind == 4) { begin_apply(e, e.ag.cur_action); return true; }  // (rlm_act already drew the action)
-  const int a = begin_select(e, mt_pol, D);
+__device__ __noinline__ void begin_apply(EnvHdr& e, int a) { begin_apply_in(e, a); }
+__device__ __noinline__ void begin_apply(EnvHdr& e, int a, EnvMarket mk) { begin_apply_in(e, a, mk); }
+template <class... M>
+__device__ __forceinline__ bool begin_step(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D, M... mk) {
+  if (e.ag.kind == 4) { begin_apply(e, e.ag.cur_action, mk...); return true; }  // (rlm_act already drew the action)
+  const int a = begin_select(e, mt_pol, D, mk...);
   if (a < 0) return false;
-  begin_apply(e, a);
+  begin_apply(e, a, mk...);
   return true;
 }
 // The same for the warp-per-env tick kernels: lane 0 selects the action and runs DoAction's book-keeping, the two quotes
 // (Intraday::l2p_ + RiskManager::PlaceOrder, intraday.cpp:64-82,163-173) are priced and placed by lane 0 (ask) and lane 1
 // (bid) side by side -- two ToTicks / ToPrice / queue look-ups instead of four in a row on the launch's critical path.
-__device__ __forceinline__ void begin_step_warp(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D, int* flag, int lane) {
+template <class... M>
+__device__ __forceinline__ void begin_step_warp(EnvHdr& e, unsigned long long* mt_pol, const DynParams& D, int* flag, int lane, M... mk) {
   if (lane == 0) {
     int a;
     if (e.ag.kind == 4) a = e.ag.cur_action;  // (rlm_act already drew the action)
-    else a = begin_select(e, mt_pol, D);
+    else a = begin_select(e, mt_pol, D, mk...);
     int place = 0;
     if (a >= 0) {
       e.ag.cur_action = a;
@@ -321,11 +337,11 @@ __device__ __forceinline__ void begin_step_warp(EnvHdr& e, unsigned long long* m
       const int lv = lane == 0 ? e.ask_level : -e.bid_level;
       double q;
       if (P.l2p_book) {
-        q = to_price(to_ticks(e.side[lane].px[0], &lerr, &hint) + lv, &lerr);
+        q = to_price(mk..., to_ticks(mk..., e.side[lane].px[0], &lerr, &hint) + lv, &lerr);
       } else {
         const double tp = e.tp_val, half_spd = fmax(0.0, e.w_mean[W_SPREAD] / 2.0);
         const double px = lane == 0 ? tp + (double)e.ask_level * half_spd : tp - (double)e.bid_level * half_spd;
-        q = to_price(to_ticks(px, &lerr, &hint), &lerr);
+        q = to_price(mk..., to_ticks(mk..., px, &lerr, &hint), &lerr);
       }
       if (lane == 0) e.ask_quote = q; else e.bid_quote = q;
       side_replace_order(e.side[lane], q, P.order_size, &lerr);
@@ -344,6 +360,25 @@ __device__ __forceinline__ void begin_step_warp(EnvHdr& e, unsigned long long* m
   if (lane == 0) e.ag.need_begin = 0;
   __syncwarp();
 }
+// The market argument of env b's tick (rlm_env.cuh, EnvMarket): MKT = false, the config's market (no argument, and no
+// load); MKT = true, the VenueD of the market of b's day.  on_market<MKT>(mk, f) calls f() or f(mk).
+template <bool MKT>
+__device__ __forceinline__ EnvMarket env_market_of(int b) {
+  EnvMarket m{nullptr};
+  if (MKT) m.v = PM.markets + PM.env_market[b];
+  return m;
+}
+template <bool MKT, class F>
+__device__ __forceinline__ decltype(auto) on_market(EnvMarket mk, F&& f) {
+  if constexpr (MKT) return f(mk);
+  else return f();
+}
+template <bool MKT>
+__device__ __forceinline__ bool env_is_terminal(const EnvHdr& e, int b) {
+  if constexpr (MKT) return is_terminal(e, env_market_of<true>(b));
+  else return is_terminal(e);
+}
+
 // split surface: is this env waiting for rlm_agent_update (its step or its warm-up has ended) or for rlm_env_step to
 // apply an action?  Such envs do not tick under DynParams::hold.
 __device__ __forceinline__ bool env_on_hold(const EnvHdr& e) {
@@ -354,6 +389,7 @@ __device__ __forceinline__ bool env_on_hold(const EnvHdr& e) {
 // Split surface (include/rlm.h: rlm_act / rlm_env_step / rlm_agent_update), one thread per env, straight on the
 // record in HBM (this is the interoperability path, not the training loop).
 // rlm_act: Agent::action for every env at a decision point; actions[b] = -1 elsewhere (and at the end of an episode).
+template <bool MKT>
 __global__ void rlm_act_kernel(DevPtrs ptr, DynParams D, int* actions) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= P.n_envs) return;
@@ -362,7 +398,7 @@ __global__ void rlm_act_kernel(DevPtrs ptr, DynParams D, int* actions) {
   if (e.phase == PH_RUN && e.ag.need_begin) {
     if (e.ag.kind == 4) a = e.ag.cur_action;  // already selected, not applied yet
     else {
-      a = begin_select(e, ptr.mt_pol + (size_t)b * 312, D);
+      a = on_market<MKT>(env_market_of<MKT>(b), [&](auto... mk) { return begin_select(e, ptr.mt_pol + (size_t)b * 312, D, mk...); });
       if (a >= 0) { e.ag.cur_action = a; e.ag.kind = 4; }
       else e.ag.need_begin = 0;
     }
@@ -371,25 +407,28 @@ __global__ void rlm_act_kernel(DevPtrs ptr, DynParams D, int* actions) {
 }
 // first half of rlm_env_step: Base::performAction(actions[b]) up to its do-while for every env at a decision point.
 // actions == nullptr: the agent's own choice (rlm_act semantics, selected here if rlm_act was not called).
+template <bool MKT>
 __global__ void rlm_apply_kernel(DevPtrs ptr, DynParams D, const int* actions) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= P.n_envs) return;
   EnvHdr& e = *(EnvHdr*)(ptr.env + (size_t)b * P.env_stride);
   if (e.phase != PH_RUN || !e.ag.need_begin) return;
+  const EnvMarket mk = env_market_of<MKT>(b);
   int a;
   if (e.ag.kind == 4) a = actions ? actions[b] : e.ag.cur_action;
   else if (actions) {  // external policy: Learner::_step without Agent::action (no generator draw)
-    if (is_terminal(e)) { clear_inventory(e); e.phase = PH_DONE; e.ag.need_begin = 0; return; }
+    if (on_market<MKT>(mk, [&](auto... m) { return is_terminal(e, m...); })) { clear_inventory(e); e.phase = PH_DONE; e.ag.need_begin = 0; return; }
     a = actions[b];
   } else {
-    a = begin_select(e, ptr.mt_pol + (size_t)b * 312, D);
+    a = on_market<MKT>(mk, [&](auto... m) { return begin_select(e, ptr.mt_pol + (size_t)b * 312, D, m...); });
     if (a < 0) { e.ag.need_begin = 0; return; }
   }
   if (a < 0 || a >= P.n_actions) { e.err |= ERR_BAD_PRICE; a = 0; }
-  begin_apply(e, a);
+  on_market<MKT>(mk, [&](auto... m) { begin_apply(e, a, m...); });
   e.ag.need_begin = 0;
 }
 // per-env outputs of rlm_env_step / rlm_agent_update
+template <bool MKT>
 __global__ void rlm_step_out_kernel(DevPtrs ptr, double* reward, unsigned char* terminal, double* delta) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= P.n_envs) return;
@@ -400,20 +439,23 @@ __global__ void rlm_step_out_kernel(DevPtrs ptr, double* reward, unsigned char* 
     // has stopped inside performAction -- the reference's performAction returning false at the end of its files
     const int2 tc = P.source == RLM_SOURCE_TAPE ? ptr.tape_cur[b] : make_int2(0, 1);
     if (e.phase != PH_DONE && !env_on_hold(e) && tc.x >= tc.y) terminal[b] = 2;
-    else terminal[b] = (e.phase == PH_DONE || (e.phase == PH_RUN && is_terminal(e))) ? 1 : 0;
+    else terminal[b] = (e.phase == PH_DONE || (e.phase == PH_RUN && env_is_terminal<MKT>(e, b))) ? 1 : 0;
   }
   if (delta) delta[b] = e.ag.last_delta;
 }
 cudaError_t rlm_launch_act(const DevPtrs& ptr, const DynParams& D, int n_envs, int* actions, cudaStream_t st) {
-  rlm_act_kernel<<<(n_envs + 63) / 64, 64, 0, st>>>(ptr, D, actions);
+  if (g_day_markets) rlm_act_kernel<true><<<(n_envs + 63) / 64, 64, 0, st>>>(ptr, D, actions);
+  else rlm_act_kernel<false><<<(n_envs + 63) / 64, 64, 0, st>>>(ptr, D, actions);
   return cudaGetLastError();
 }
 cudaError_t rlm_launch_apply(const DevPtrs& ptr, const DynParams& D, int n_envs, const int* actions, cudaStream_t st) {
-  rlm_apply_kernel<<<(n_envs + 63) / 64, 64, 0, st>>>(ptr, D, actions);
+  if (g_day_markets) rlm_apply_kernel<true><<<(n_envs + 63) / 64, 64, 0, st>>>(ptr, D, actions);
+  else rlm_apply_kernel<false><<<(n_envs + 63) / 64, 64, 0, st>>>(ptr, D, actions);
   return cudaGetLastError();
 }
 cudaError_t rlm_launch_step_out(const DevPtrs& ptr, int n_envs, double* reward, unsigned char* terminal, double* delta, cudaStream_t st) {
-  rlm_step_out_kernel<<<(n_envs + 127) / 128, 128, 0, st>>>(ptr, reward, terminal, delta);
+  if (g_day_markets) rlm_step_out_kernel<true><<<(n_envs + 127) / 128, 128, 0, st>>>(ptr, reward, terminal, delta);
+  else rlm_step_out_kernel<false><<<(n_envs + 127) / 128, 128, 0, st>>>(ptr, reward, terminal, delta);
   return cudaGetLastError();
 }
 
@@ -518,26 +560,27 @@ __device__ __noinline__ void flow_next_warp(rlm_flow_state* s, rlm_tick_msg* m, 
 
 // One market tick of one env (thread-per-env).  Returns -1, or the ready kind: 0 = a learner step
 // ended (state variables + reward are in e.ag), 1 = warm-up ended (Intraday::Initialise done).
-__device__ __noinline__ int env_tick(EnvHdr& e, double* ring, const rlm_tick_msg& msg, int backtest) {
+template <class... M>
+__device__ __forceinline__ int env_tick_in(EnvHdr& e, double* ring, const rlm_tick_msg& msg, int backtest, M... mk) {
   const int phase = e.phase;
   const bool multi = needs_multi(e, msg);  // ingested real data: this tick spans several messages (rlm_flow.h)
   if (phase == PH_PREOPEN) {  // intraday.cpp:111-116: rows before the open only update the book
     if (multi) {
-      if (update_book_profiles_multi(e, msg, false) && market_is_open(e)) e.phase = PH_WARMUP;
+      if (update_book_profiles_multi(e, msg, false) && market_is_open(e, mk...)) e.phase = PH_WARMUP;
       return -1;
     }
     rlm_tick_msg none = msg;
     none.n_tx = 0;
     update_book_profiles(e, none);
-    if (market_is_open(e)) e.phase = PH_WARMUP;
+    if (market_is_open(e, mk...)) e.phase = PH_WARMUP;
     return -1;
   }
   double pushv[RLM_NWIN], oldv[RLM_NWIN];
 #pragma unroll
   for (int w = 0; w < RLM_NWIN; ++w) oldv[w] = window_peek(e, ring, w);  // 10 independent loads, consumed after the book logic
   if (phase == PH_RUN) e.pnl_step = 0.0;  // base.cpp:286
-  if (multi) { if (!next_state_multi(e, msg, pushv)) return -2; }  // (message consumed, tick not complete yet)
-  else next_state_scalar(e, msg, pushv);  // Intraday::NextState
+  if (multi) { if (!next_state_multi(e, msg, pushv, mk...)) return -2; }  // (message consumed, tick not complete yet)
+  else next_state_scalar(e, msg, pushv, mk...);  // Intraday::NextState
 #pragma unroll 1
   for (int w = 0; w < 8; ++w) window_push(e, ring, w, pushv[w], oldv[w]);
   e.tp_val = e.w_mean[W_TP];
@@ -546,12 +589,12 @@ __device__ __noinline__ int env_tick(EnvHdr& e, double* ring, const rlm_tick_msg
 #pragma unroll 1
     for (int w = 0; w < 8; ++w) full = full && (e.w_count[w] == P.win_size[w]);
     if (!full) return -1;
-    place_orders(e, 1, 1);
+    place_orders(e, 1, 1, mk...);
     e.phase = PH_RUN;
     e.ag.kind = 1;  // serial.cpp:24-25,55-60: the first from-state is the never-populated State
     if (backtest) {  // Backtester::_step builds its state from the env before every action (serial.cpp:126)
 #pragma unroll 1
-      for (int i = 0; i < P.n_state_vars; ++i) e.ag.to_vars[i] = (float)get_variable(e, ring, P.state_vars[i]);
+      for (int i = 0; i < P.n_state_vars; ++i) e.ag.to_vars[i] = (float)get_variable(e, ring, P.state_vars[i], mk...);
     }
     return 1;
   }
@@ -562,7 +605,7 @@ __device__ __noinline__ int env_tick(EnvHdr& e, double* ring, const rlm_tick_msg
   e.agg_r += get_reward(e);
   e.agg_pnl += e.pnl_step;
   e.agg_mpm += mpm;
-  if (!is_terminal(e) && fabs(e.agg_mpm) < 1e-5) return -1;
+  if (!is_terminal(e, mk...) && fabs(e.agg_mpm) < 1e-5) return -1;
   // base.cpp:317-331
   e.pnl_step = e.agg_pnl;
   window_push(e, ring, W_PNLUP, fmax(0.0, e.pnl_step), oldv[W_PNLUP]);
@@ -571,15 +614,21 @@ __device__ __noinline__ int env_tick(EnvHdr& e, double* ring, const rlm_tick_msg
   e.ep_bandh += e.agg_mpm;
   // State::newState -> Intraday::getState (state.cpp:35-43, intraday.cpp:411-416); serial.cpp:64-65
 #pragma unroll 1
-  for (int i = 0; i < P.n_state_vars; ++i) e.ag.to_vars[i] = (float)get_variable(e, ring, P.state_vars[i]);
+  for (int i = 0; i < P.n_state_vars; ++i) e.ag.to_vars[i] = (float)get_variable(e, ring, P.state_vars[i], mk...);
   e.ag.last_reward = get_reward(e);
   e.ag.kind = 0;
   e.ag.hs_valid = 0;  // (one thread per env: the learner kernel hashes the to-state itself)
   return 0;
 }
 
-// TAPE: instantiation for the tape source (the other sources' code is the same as without it)
-template <int THREADS, bool TAPE>
+__device__ __noinline__ int env_tick(EnvHdr& e, double* ring, const rlm_tick_msg& msg, int backtest) { return env_tick_in(e, ring, msg, backtest); }
+__device__ __noinline__ int env_tick(EnvHdr& e, double* ring, const rlm_tick_msg& msg, int backtest, EnvMarket mk) {
+  return env_tick_in(e, ring, msg, backtest, mk);
+}
+
+// TAPE: instantiation for the tape source (the other sources' code is the same as without it); MKT: ... whose days run
+// under markets of their own (rlm_set_day_markets)
+template <int THREADS, bool TAPE, bool MKT = false>
 __global__ void __launch_bounds__(THREADS) rlm_env_kernel(DevPtrs ptr, DynParams D, int tslot, int only_begin) {
   const int b = D.env0 + blockIdx.x * THREADS + threadIdx.x;
   const int lane = threadIdx.x & 31;
@@ -591,6 +640,7 @@ __global__ void __launch_bounds__(THREADS) rlm_env_kernel(DevPtrs ptr, DynParams
     EnvHdr* g = (EnvHdr*)(ptr.env + (size_t)b * P.env_stride);
     // tape source: the cursor comes from its own array, so its load is in flight together with the record copy below
     const int2 tc = (TAPE && !only_begin) ? ptr.tape_cur[b] : make_int2(0, 0);
+    const EnvMarket mk = env_market_of<MKT>(b);
     const int ph = g->phase;
     const int nb = D.hold ? 0 : g->ag.need_begin;
     if (ph != PH_DONE && (!only_begin || nb) && !(D.hold && env_on_hold(*g))) {
@@ -609,7 +659,7 @@ __global__ void __launch_bounds__(THREADS) rlm_env_kernel(DevPtrs ptr, DynParams
       }
       double* ring = (double*)((unsigned char*)g + sizeof(EnvHdr));
       if (nb) {
-        begin_step(e, ptr.mt_pol + (size_t)b * 312, D);
+        on_market<MKT>(mk, [&](auto... m) { begin_step(e, ptr.mt_pol + (size_t)b * 312, D, m...); });
         e.ag.need_begin = 0;
       }
       if (!only_begin && e.phase != PH_DONE) {
@@ -648,7 +698,7 @@ __global__ void __launch_bounds__(THREADS) rlm_env_kernel(DevPtrs ptr, DynParams
         }
         if (have) {
           const int was = e.phase;
-          ready = env_tick(e, ring, msg, D.backtest);
+          ready = on_market<MKT>(mk, [&](auto... m) { return env_tick(e, ring, msg, D.backtest, m...); });
           if (was != PH_PREOPEN && ready != -2) ticked = 1;
           if (ready == -2) ready = -1;
         }
@@ -774,9 +824,9 @@ __device__ __forceinline__ void envw_stage_out(EnvHdr* g, const EnvHdr* src_e, i
 // Tape source: stream_pos / stream_ticks are the env's cursor and the end of its day, and tape_word is this lane's word of
 // message stream_pos, loaded by the caller ahead of the record's stage-in.
 // Returns -1, or the ready kind (0: a learner step ended -- state variables and reward are in e.ag; 1: warm-up ended).
-template <bool TAPE = false>
+template <bool TAPE = false, class... M>
 __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const DevPtrs& ptr, const DynParams& D, int env, int stream_pos,
-                                         int stream_ticks, int lane, unsigned& ticked, unsigned tape_word = 0) {
+                                         int stream_ticks, int lane, unsigned& ticked, unsigned tape_word = 0, M... mk) {
   EnvHdr& e = *w.e;
   rlm_tick_msg& msg = *w.msg;
   double* pushv = w.pushv;
@@ -800,18 +850,18 @@ __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const D
   if (multi && phase != PH_PREOPEN) {  // lane 0 runs the one-thread version; the tick may not be complete yet
     if (lane == 0) {
       if (phase == PH_RUN) e.pnl_step = 0.0;  // base.cpp:286
-      complete = next_state_multi(e, msg, pushv) ? 1 : 0;
+      complete = next_state_multi(e, msg, pushv, mk...) ? 1 : 0;
     }
     complete = __shfl_sync(FULL, complete, 0);
   }
   if (have && phase == PH_PREOPEN) {  // intraday.cpp:111-116
     if (lane == 0) {
       if (multi) {
-        if (update_book_profiles_multi(e, msg, false) && market_is_open(e)) e.phase = PH_WARMUP;
+        if (update_book_profiles_multi(e, msg, false) && market_is_open(e, mk...)) e.phase = PH_WARMUP;
       } else {
         msg.n_tx = 0;
         update_book_profiles(e, msg);
-        if (market_is_open(e)) e.phase = PH_WARMUP;
+        if (market_is_open(e, mk...)) e.phase = PH_WARMUP;
       }
     }
   } else if (have && complete) {
@@ -819,7 +869,7 @@ __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const D
     if (!multi) {
       if (lane == 0 && phase == PH_RUN) e.pnl_step = 0.0;  // base.cpp:286
       __syncwarp();
-      next_state_warp(e, msg, pushv, w.fills, lane);  // Intraday::NextState, ask side on lane 0, bid side on lane 1
+      next_state_warp(e, msg, pushv, w.fills, lane, mk...);  // Intraday::NextState, ask side on lane 0, bid side on lane 1
     }
     __syncwarp();
     if (lane < 8) window_push(e, ring, lane, pushv[lane], oldv[lane]);
@@ -831,7 +881,7 @@ __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const D
         bool full = true;
         for (int k = 0; k < 8; ++k) full = full && (e.w_count[k] == P.win_size[k]);
         if (full) {
-          place_orders(e, 1, 1);
+          place_orders(e, 1, 1, mk...);
           e.phase = PH_RUN;
           e.ag.kind = 1;  // serial.cpp:24-25,55-60: the first from-state is the never-populated (or the stale) State
           r = 1;
@@ -844,7 +894,7 @@ __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const D
         e.agg_r += get_reward(e);
         e.agg_pnl += e.pnl_step;
         e.agg_mpm += mpm;
-        if (!(!is_terminal(e) && fabs(e.agg_mpm) < 1e-5)) {
+        if (!(!is_terminal(e, mk...) && fabs(e.agg_mpm) < 1e-5)) {
           e.pnl_step = e.agg_pnl;  // base.cpp:317-331
           pushv[W_PNLUP] = fmax(0.0, e.pnl_step);
           pushv[W_PNLDN] = fabs(fmin(0.0, e.pnl_step));
@@ -870,9 +920,9 @@ __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const D
         double x0 = 0.0, x1 = 0.0;
         const bool two = has && var_tick_args(e, ring, var, x0, x1);
         int t0 = 0, t1 = 0, lerr = 0, hint = e.tk_band;
-        if (two) { t0 = to_ticks(x0, &lerr, &hint); t1 = to_ticks(x1, &lerr, &hint); }
+        if (two) { t0 = to_ticks(mk..., x0, &lerr, &hint); t1 = to_ticks(mk..., x1, &lerr, &hint); }
         if (lerr) atomicOr(&e.err, lerr);
-        if (has) e.ag.to_vars[lane] = (float)(two ? var_from_ticks(var, t0, t1) : get_variable(e, ring, var));
+        if (has) e.ag.to_vars[lane] = (float)(two ? var_from_ticks(var, t0, t1) : get_variable(e, ring, var, mk...));
       }
       if (lane == 31) { e.ag.last_reward = get_reward(e); e.ag.kind = 0; }
       if (D.env_hash && !D.backtest && !P.shared_policy && P.algorithm < RLM_ALGO_R_LEARN) {
@@ -901,14 +951,14 @@ __device__ __forceinline__ int envw_tick(const EnvWarp& w, double* ring, const D
       }
     } else if (ready == 1 && D.backtest) {
       // Backtester::_step builds its state from the env before every action (serial.cpp:126), the first one included
-      if (lane < P.n_state_vars) e.ag.to_vars[lane] = (float)get_variable(e, ring, P.state_vars[lane]);
+      if (lane < P.n_state_vars) e.ag.to_vars[lane] = (float)get_variable(e, ring, P.state_vars[lane], mk...);
     }
   }
   __syncwarp();
   return ready;
 }
 
-template <bool TAPE>
+template <bool TAPE, bool MKT = false>
 __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr, DynParams D, int tslot, int only_begin) {
   PDL_PROLOGUE();
   extern __shared__ __align__(16) unsigned char smem[];
@@ -923,6 +973,7 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr,
   // the trailing begin-only pass touches few envs: look before staging.  A tick pass stages straight away -- one
   // memory round trip instead of two on every env's critical path -- and drops finished envs afterwards.
   if (only_begin && !g->ag.need_begin) return;
+  const EnvMarket mk = env_market_of<MKT>(env);
   const bool tape = TAPE && !only_begin;
   int2 tc = make_int2(0, 0);
   unsigned tape_word = 0;
@@ -934,12 +985,12 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr,
   int ready = -1;
   unsigned ticked = 0;
   bool starved = false;  // tape source: this env needs a message past the end of its day
-  if (e.ag.need_begin) begin_step_warp(e, ptr.mt_pol + (size_t)env * 312, D, w.flag, lane);
+  if (e.ag.need_begin) on_market<MKT>(mk, [&](auto... m) { begin_step_warp(e, ptr.mt_pol + (size_t)env * 312, D, w.flag, lane, m...); });
   if (!only_begin && e.phase != PH_DONE) {
     if (tape) {
       starved = tc.x >= tc.y;
       if (!starved) {
-        ready = envw_tick<true>(w, ring, ptr, D, env, tc.x, tc.y, lane, ticked, tape_word);
+        ready = on_market<MKT>(mk, [&](auto... m) { return envw_tick<true>(w, ring, ptr, D, env, tc.x, tc.y, lane, ticked, tape_word, m...); });
         if (lane == 0) ptr.tape_cur[env].x = tc.x + 1;
       }
     } else if (D.ctl_stream) {  // (see rlm_env_kernel: stream pointer, offset and length of this call live in *ptr.runctl)
@@ -969,7 +1020,7 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32) rlm_env_kernel_w(DevPtrs ptr,
 // instead of once per market tick.  Envs never exchange anything (own book, own stream, own weights), so the order in
 // which their ticks run is not observable: per env the sequence begin_step / tick / ... / learner step is the same as
 // in the tick-synchronous engine, bit for bit.  The per-call values live in *ptr.runctl (graphs are reused across calls).
-template <bool TAPE>
+template <bool TAPE, bool MKT = false>
 __global__ void __launch_bounds__(ENVW_WARPS * 32, 4) rlm_env_round_kernel(DevPtrs ptr, DynParams D, int tslot) {
   PDL_PROLOGUE();
   extern __shared__ __align__(16) unsigned char smem[];
@@ -990,6 +1041,7 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32, 4) rlm_env_round_kernel(DevPt
   EnvHdr* g = (EnvHdr*)(ptr.env + (size_t)env * P.env_stride);
   double* ring = (double*)((unsigned char*)g + sizeof(EnvHdr));
   const bool tape = TAPE;
+  const EnvMarket mk = env_market_of<MKT>(env);
   int2 tc = make_int2(0, 0);
   unsigned tape_word = 0;
   if (tape) tape_word = envw_stage_in_tape(&e, g, ptr, env, lane, false, tc);
@@ -1007,13 +1059,13 @@ __global__ void __launch_bounds__(ENVW_WARPS * 32, 4) rlm_env_round_kernel(DevPt
   bool starved = false;  // tape source: the env's day has run out (it waits inside performAction, consuming nothing)
 #pragma unroll 1
   for (;;) {
-    if (e.ag.need_begin) begin_step_warp(e, ptr.mt_pol + (size_t)env * 312, D, w.flag, lane);
+    if (e.ag.need_begin) on_market<MKT>(mk, [&](auto... m) { begin_step_warp(e, ptr.mt_pol + (size_t)env * 312, D, w.flag, lane, m...); });
     if (e.phase == PH_DONE || pos >= rc.n_ticks || n_run >= cap) break;
     if (tape) {
       if (tc.x >= tc.y) { starved = true; break; }
       const unsigned word = tape_word;
       if (tc.x + 1 < tc.y) tape_word = __ldg((const unsigned*)(ptr.tape + tc.x + 1) + lane);  // the next tick's, in flight during this one
-      ready = envw_tick<true>(w, ring, pt, D, env, tc.x, tc.y, lane, ticked, word);
+      ready = on_market<MKT>(mk, [&](auto... m) { return envw_tick<true>(w, ring, pt, D, env, tc.x, tc.y, lane, ticked, word, m...); });
       ++tc.x;
     } else {
       ready = envw_tick(w, ring, pt, D, env, rc.stream_off + pos, rc.stream_ticks, lane, ticked);
@@ -2031,25 +2083,26 @@ static int envw_carveout() {
 cudaError_t rlm_launch_env(const DevPtrs& ptr, const DynParams& D, int n_envs, int tslot, int only_begin, int variant, cudaStream_t st) {
   if (D.n_sub > 0) n_envs = D.n_sub;  // one sub-batch
   const bool tape = ptr.tape_cur != nullptr;  // (the cursors exist on the tape source only)
+  const int kv = g_day_markets ? 2 : (tape ? 1 : 0);  // instantiation: generator / stream, tape, tape with day markets
   if (variant == 1) {  // one thread per env (SIMT over envs)
     const int T = 32;
-    static bool attr1[2] = {false, false};
-    if (!attr1[tape]) {
+    auto kern = kv == 2 ? rlm_env_kernel<T, true, true> : (kv == 1 ? rlm_env_kernel<T, true> : rlm_env_kernel<T, false>);
+    static bool attr1[3] = {false, false, false};
+    if (!attr1[kv]) {
       // this kernel uses no shared memory at all; its per-thread record copy lives in local memory, i.e. in L1 (RLM_ENVT_CARVEOUT)
       int c = RLM_ENVT_CARVEOUT_DEFAULT;
       if (const char* e = getenv("RLM_ENVT_CARVEOUT")) { const int v = atoi(e); if (v >= 0 && v <= 100) c = v; }
-      cudaFuncSetAttribute(tape ? rlm_env_kernel<T, true> : rlm_env_kernel<T, false>, cudaFuncAttributePreferredSharedMemoryCarveout, c);
-      attr1[tape] = true;
+      cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, c);
+      attr1[kv] = true;
     }
-    if (tape) rlm_env_kernel<T, true><<<(n_envs + T - 1) / T, T, 0, st>>>(ptr, D, tslot, only_begin);
-    else rlm_env_kernel<T, false><<<(n_envs + T - 1) / T, T, 0, st>>>(ptr, D, tslot, only_begin);
+    kern<<<(n_envs + T - 1) / T, T, 0, st>>>(ptr, D, tslot, only_begin);
     return cudaGetLastError();
   }
   const int W = envw_warps_per_cta();
   const size_t smem = (size_t)W * envw_warp_bytes();
-  auto kern = tape ? rlm_env_kernel_w<true> : rlm_env_kernel_w<false>;
-  static bool attr[2] = {false, false};
-  if (!attr[tape]) {
+  auto kern = kv == 2 ? rlm_env_kernel_w<true, true> : (kv == 1 ? rlm_env_kernel_w<true> : rlm_env_kernel_w<false>);
+  static bool attr[3] = {false, false, false};
+  if (!attr[kv]) {
     if (smem > 48 * 1024) {
       cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
@@ -2057,7 +2110,7 @@ cudaError_t rlm_launch_env(const DevPtrs& ptr, const DynParams& D, int n_envs, i
     // the same L1/shared split as the learner kernel: CTAs of the two kernels (different sub-batches, different streams)
     // can then share an SM instead of waiting for it to drain and be reconfigured
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, envw_carveout());
-    attr[tape] = true;
+    attr[kv] = true;
   }
   return launch_pdl(kern, (n_envs + W - 1) / W, W * 32, smem, st, ptr, D, tslot, only_begin);
 }
@@ -2066,15 +2119,16 @@ cudaError_t rlm_launch_env_round(const DevPtrs& ptr, const DynParams& D, int n_e
   const int W = envw_warps_per_cta();
   const size_t smem = (size_t)W * envw_warp_bytes();
   const bool tape = ptr.tape_cur != nullptr;
-  auto kern = tape ? rlm_env_round_kernel<true> : rlm_env_round_kernel<false>;
-  static bool attr[2] = {false, false};
-  if (!attr[tape]) {
+  const int kv = g_day_markets ? 2 : (tape ? 1 : 0);  // (as in rlm_launch_env)
+  auto kern = kv == 2 ? rlm_env_round_kernel<true, true> : (kv == 1 ? rlm_env_round_kernel<true> : rlm_env_round_kernel<false>);
+  static bool attr[3] = {false, false, false};
+  if (!attr[kv]) {
     if (smem > 48 * 1024) {
       cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
     }
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, envw_carveout());
-    attr[tape] = true;
+    attr[kv] = true;
   }
   return launch_pdl(kern, (n_envs + W - 1) / W, W * 32, smem, st, ptr, D, tslot);
 }
@@ -2117,6 +2171,48 @@ cudaError_t rlm_launch_gather(const DevPtrs& ptr, int n_envs, int what, void* ou
 }
 cudaError_t rlm_launch_clear_traces(const DevPtrs& ptr, int n_envs, cudaStream_t st) {
   rlm_clear_traces_kernel<<<(n_envs + 127) / 128, 128, 0, st>>>(ptr);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------
+// Day markets (rlm_set_day_markets).  Envs env0 .. env0+n-1 take markets mk[0..n-1] (-1: the config's; the host launches
+// this only when some env's market changes, or the markets themselves were replaced) and forget next_state_tail's
+// midprice memo: it holds ToTicks under the old table, and the next day may open at
+// the same midprice.  (The band hint needs no clearing: to_ticks checks it against the table, whose unused bands are +inf.)
+__global__ void rlm_env_market_kernel(DevPtrs ptr, int env0, int n, const int* mk) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int b = env0 + i;
+  PM.env_market[b] = mk[i];
+  EnvHdr* e = (EnvHdr*)(ptr.env + (size_t)b * P.env_stride);
+  e->tk_px = 0.0;
+  e->tk_ticks = 0;
+}
+cudaError_t rlm_launch_env_market(const DevPtrs& ptr, int env0, int n, const int* mk, cudaStream_t st) {
+  rlm_env_market_kernel<<<(n + 127) / 128, 128, 0, st>>>(ptr, env0, n, mk);
+  return cudaGetLastError();
+}
+// Under day markets the learner kernels fill a record's terminal flag from the config's market, which the host then sets
+// to never close (rlm_api.cu, day_markets_on): the flag they write is the date change of Intraday::isTerminal alone.  This
+// kernel adds the env's own market's close to the records written since it last ran (every record env, one thread each);
+// the host runs it before an env's market changes and before records are read.
+__global__ void rlm_fix_terminal_kernel(DevPtrs ptr) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= P.record_envs) return;
+  const int n = min(ptr.record_count[b], P.record_cap);
+  const int k = PM.env_market[b];  // (-1 only between the first rlm_set_day_markets and its assignment, with no record due)
+  if (k >= 0) {
+    const VenueD* V = PM.markets + k;
+    for (int i = PM.rec_fixed[b]; i < n; ++i) {
+      rlm_step_record& r = ptr.records[(size_t)b * P.record_cap + i];
+      if (!((long long)r.time_ms > V->open_lo && (long long)r.time_ms < V->close_hi)) r.terminal = 1;
+    }
+  }
+  PM.rec_fixed[b] = max(n, PM.rec_fixed[b]);
+}
+cudaError_t rlm_launch_fix_terminal(const DevPtrs& ptr, int record_envs, cudaStream_t st) {
+  if (record_envs <= 0) return cudaSuccess;
+  rlm_fix_terminal_kernel<<<(record_envs + 127) / 128, 128, 0, st>>>(ptr);
   return cudaGetLastError();
 }
 

@@ -5,7 +5,7 @@
 
 size_t rlm_scratch_bytes(int is_double);
 size_t rlm_agent_smem_bytes(int warps_per_cta, int scratch_bytes);
-cudaError_t rlm_upload_params(const DevParams* p);
+cudaError_t rlm_upload_params(const DevParams* p, const DevMarkets* m);
 cudaError_t rlm_launch_env(const DevPtrs& ptr, const DynParams& D, int n_envs, int tslot, int only_begin, int variant, cudaStream_t st);
 cudaError_t rlm_launch_env_round(const DevPtrs& ptr, const DynParams& D, int n_envs, int tslot, cudaStream_t st);
 cudaError_t rlm_launch_runctl(const DevPtrs& ptr, const RunCtl& v, cudaStream_t st);
@@ -32,6 +32,8 @@ cudaError_t rlm_launch_random_init(const DevPtrs& ptr, int n_policies, cudaStrea
 void rlm_set_pdl(int on);
 cudaError_t rlm_launch_gather(const DevPtrs& ptr, int n_envs, int what, void* out, cudaStream_t st);
 cudaError_t rlm_launch_clear_traces(const DevPtrs& ptr, int n_envs, cudaStream_t st);
+cudaError_t rlm_launch_env_market(const DevPtrs& ptr, int env0, int n, const int* mk, cudaStream_t st);
+cudaError_t rlm_launch_fix_terminal(const DevPtrs& ptr, int record_envs, cudaStream_t st);
 cudaError_t rlm_launch_test_to_ticks(const double* px, int n, int* out);
 cudaError_t rlm_launch_test_to_price(const int* t, int n, double* out);
 cudaError_t rlm_launch_test_tiles(const float* vars, int n, int* out);

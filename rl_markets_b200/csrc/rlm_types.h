@@ -199,3 +199,11 @@ struct DevPtrs {
   int2* tape_cur;                // [n_envs] {next message, end of the env's day} (absolute message indices)
   int* tape_lo;                  // [n_envs] first message of the env's day (rlm_reset / rlm_new_env rewind to it)
 };
+
+// Tape days with markets of their own (rlm_set_day_markets).  A __constant__ block of its own (rlm_env.cuh: PM), uploaded
+// with DevParams: only the kernels that read an env's market see it, every other kernel keeps its parameters.
+struct DevMarkets {
+  const VenueD* markets;  // [n_markets]; null while every day runs under the config's market
+  int* env_market;        // [n_envs] market of the env's current day (-1: the config's)
+  int* rec_fixed;         // [record_envs] records whose terminal flag already accounts for the env's market
+};

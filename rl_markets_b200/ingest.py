@@ -78,6 +78,23 @@ def day_library(samples):
     return out, offsets
 
 
+def day_markets(samples):
+    """The (symbol, md csv, tas csv) tuples of file_sample / sample_window -> (markets, day_market) for
+    BatchedMarket.set_day_markets: day d runs under markets[day_market[d]], its symbol's market (config.market), as
+    Intraday::LoadData builds it from the ticker (src/environment/intraday.cpp:141-150).  Markets are deduplicated by tick
+    table and trading hours, in first-seen order."""
+    from . import config
+    markets, day_market = [], []
+    for symbol, _md, _tas in samples:
+        m = config.market(symbol)
+        k = next((i for i, o in enumerate(markets) if config.same_market(o, m)), None)
+        if k is None:
+            k = len(markets)
+            markets.append(m)
+        day_market.append(k)
+    return markets, day_market
+
+
 def load_day(market, md_path, tas_path):
     """Intraday::LoadData (src/environment/intraday.cpp:141-150) for every env of a STREAM-source handle: the same day for
     all of them.  Returns the number of message slots to pass to run_ticks."""

@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get("RLM_LIB_PATH") or os.path.join(_HERE, "librlm.so")  #
 
 EXPORTS = [
     "rlm_last_error", "rlm_abi_version", "rlm_config_default", "rlm_create", "rlm_destroy", "rlm_reset", "rlm_set_mode", "rlm_new_env",
-    "rlm_load_ticks", "rlm_load_days", "rlm_assign_days", "rlm_get_tape_pos", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
+    "rlm_load_ticks", "rlm_load_days", "rlm_assign_days", "rlm_get_tape_pos", "rlm_set_day_markets", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
     "rlm_get_reward", "rlm_get_actions", "rlm_get_rho", "rlm_get_occupancy", "rlm_copy_theta", "rlm_handle_terminal", "rlm_go_greedy", "rlm_read_theta",
     "rlm_write_theta", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
     "rlm_set_stream", "rlm_set_profiling", "rlm_get_kernel_times", "rlm_act", "rlm_env_step", "rlm_agent_update", "rlm_ingest_csv",
@@ -54,6 +54,7 @@ def load():
     L.rlm_load_days.argtypes = [C.c_void_p, C.c_void_p, P(C.c_int64), C.c_int32]
     L.rlm_assign_days.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_int32)]
     L.rlm_get_tape_pos.argtypes = [C.c_void_p, P(C.c_int64)]
+    L.rlm_set_day_markets.argtypes = [C.c_void_p, P(abi.Market), C.c_int32, P(C.c_int32), C.c_int32]
     L.rlm_run_ticks.argtypes = [C.c_void_p, C.c_int32]
     L.rlm_sync.argtypes = [C.c_void_p]
     L.rlm_get_counters.argtypes = [C.c_void_p, P(abi.Counters)]
@@ -169,6 +170,26 @@ class BatchedMarket:
         """Tape source: env env0 + i replays day days[i] from its first message (Intraday::LoadData per env)."""
         n = len(days)
         check(self.L.rlm_assign_days(self.h, env0, n, (C.c_int32 * max(n, 1))(*days)))
+
+    def set_day_markets(self, markets, day_market):
+        """Tape source: day d runs under markets[day_market[d]] (abi.Market, e.g. config.market(ticker)); rewinds every env
+        to the start of its day, follow with reset().  A later load_days drops them (rlm_set_day_markets)."""
+        arr = (abi.Market * max(len(markets), 1))(*markets)
+        dm = (C.c_int32 * max(len(day_market), 1))(*day_market)
+        check(self.L.rlm_set_day_markets(self.h, arr, len(markets), dm, len(day_market)))
+
+    def load_day_library(self, samples):
+        """Tape source: the (symbol, md csv, tas csv) days of ingest.file_sample / sample_window into this handle, each
+        under its symbol's market.  Day markets are set only when some day's market differs from the config's, so a
+        library of one market keeps the kernels without day markets.  Returns the number of days."""
+        from . import config, ingest
+        msgs, offsets = ingest.day_library(samples)
+        self.load_days(msgs, offsets)
+        markets, day_market = ingest.day_markets(samples)
+        mine = config.config_market(self.cfg)
+        if not all(config.same_market(m, mine) for m in markets):
+            self.set_day_markets(markets, day_market)
+        return len(samples)
 
     def tape_pos(self):
         """Tape source: messages of its day each env has consumed since it was assigned or rewound."""

@@ -341,8 +341,42 @@ def reference_checks():
         json.dump(pairing, f, indent=1)
 
 
+# One tape library of all nine venue days under one yaml (the config's market is AAL.L's): env b replays day b under its
+# ticker's market (rlm_set_day_markets) with seed random_seed + DAY_MARKETS_ENV0 + b, as ref_driver --symbol <ticker> does.
+# Written to tests/golden/day_markets.json and digests_daymkt_<case>.bin, not into manifest.json, whose entries without a
+# known flag join the single-episode tests.
+DAY_MARKETS_ENV0 = 60
+
+
+def day_markets_yaml():
+    return config.example_dict(**{"learning.memory_size": 8192, "learning.algorithm": "q_learn", "data.symbols": ["AAL.L"]})
+
+
+def day_market_fixtures():
+    import tempfile
+    import golden_util
+    import test_venue_days
+    y = day_markets_yaml()
+    days = []
+    for b, c in enumerate(golden_util.venue_manifest()):
+        case = dict(c, env=DAY_MARKETS_ENV0 + b)
+        with tempfile.TemporaryDirectory() as d:
+            md, tas = golden_util.venue_day(c, d)
+            raw, summary = test_venue_days.reference_on_day(ol, case, y, md, tas, d)
+        recs = list((abi.StepRecord * (len(raw) // C.sizeof(abi.StepRecord))).from_buffer_copy(raw))
+        assert summary["terminal"] == 1 and len(recs) == summary["steps"]
+        name = "daymkt_" + c["name"]
+        _write_digests(name, recs)
+        days.append(dict(name=name, venue_case=c["name"], ticker=c["ticker"], env=DAY_MARKETS_ENV0 + b, n_records=len(recs),
+                         summary=summary))
+    with open(os.path.join(GOLD, "day_markets.json"), "w") as f:
+        json.dump(dict(yaml=y, env0=DAY_MARKETS_ENV0, days=days), f, indent=1)
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["--reference-checks"]:
         reference_checks()
+    elif sys.argv[1:] == ["--day-markets"]:
+        day_market_fixtures()
     else:
         main()
