@@ -13,6 +13,7 @@
  *   rlm_load_days         Intraday::LoadData for a library of days          src/environment/intraday.cpp:141-150
  *   rlm_assign_days       ... and which day each env replays                 src/main.cpp:45-80 (sample a day per episode)
  *   rlm_set_day_markets   ... under the market of the day's ticker          src/environment/intraday.cpp:141-150
+ *   rlm_set_flow          ... of another synthetic day, on the same env objects src/environment/intraday.cpp:141-150
  *   rlm_reset             Intraday::Initialise                             src/environment/intraday.cpp:103-138
  *   rlm_run_ticks         experiment::serial::Learner::_step               src/experiment/serial.cpp:53-70
  *                         = Agent::action + Base::performAction + State::newState
@@ -176,9 +177,22 @@ int rlm_set_mode(rlm_handle h, int32_t mode);
 
 /* `environment::Intraday<> env(c)` of src/main.cpp:219: every env object is rebuilt from scratch (window sums,
  * statistics, position, book, records) while the agents keep theta, traces, generator positions and schedules.
- * `flow` (may be NULL = keep) replaces the synthetic-flow parameters, i.e. "LoadData of another day" (generator source;
- * a tape handle takes NULL only and changes days with rlm_assign_days). */
+ * `flow` (may be NULL = keep) replaces the synthetic-flow parameters of the new object's first day (generator source;
+ * a tape handle takes NULL only and changes days with rlm_assign_days).
+ * main.cpp:219-241 builds that object ONCE and evaluates every test day on it, so rlm_new_env stands for the FIRST test
+ * day only.  Each later day is LoadData + Initialise on the same env objects, which keep what Base::Initialise does not
+ * clear (the window sums of Accumulator::clear / RollingMean, position, the experiment statistics) -- per source:
+ *   generator  rlm_set_flow(h, &next_day) + rlm_reset(h)
+ *   stream     rlm_reset(h) + rlm_load_ticks(h, next_day, n)
+ *   tape       rlm_assign_days(h, 0, n_envs, next_days) + rlm_reset(h)
+ * (A new env object per test day is what one reference process per test day computes, not main.cpp's sequence.) */
 int rlm_new_env(rlm_handle h, const rlm_flow_params* flow);
+
+/* RLM_SOURCE_GENERATOR only: Intraday::LoadData of another synthetic day (intraday.cpp:141-150) -- `flow` replaces the
+ * synthetic-flow parameters and nothing else changes; follow with rlm_reset (Initialise), which starts every env on the
+ * new day.  The call waits for the handle's work.  Stream handles load the next day with rlm_load_ticks, tape handles
+ * with rlm_assign_days (RLM_ERR_INVALID_ARGUMENT here). */
+int rlm_set_flow(rlm_handle h, const rlm_flow_params* flow);
 
 /* RLM_SOURCE_STREAM only: append `n_ticks` messages per env, host layout msgs[t][env] (tick-major).
  * The copy is issued on the handle's copy stream; the buffer must stay valid until rlm_sync. */

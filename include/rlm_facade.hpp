@@ -54,8 +54,14 @@ namespace environment {
 class Intraday {
  public:
   explicit Intraday(Session& s) : s_(s) {}
-  // Intraday::LoadData (intraday.cpp:141-150): the synthetic day is part of the config; a new day = rlm_new_env
-  void LoadData(const rlm_flow_params* day = nullptr) { if (day) check(rlm_new_env(s_.handle(), day)); }
+  // Intraday::LoadData (intraday.cpp:141-150): the synthetic day is part of the config; another day replaces its flow
+  // parameters on the same env objects (rlm_set_flow), and Initialise() starts it.  The env keeps what Initialise does
+  // not clear, as the reference's does from one test day to the next (main.cpp:219-241).
+  void LoadData(const rlm_flow_params* day = nullptr) {
+    if (!day) return;
+    check(rlm_set_flow(s_.handle(), day));
+    started_ = true;  // (the next Initialise resets the envs onto the new day's flow)
+  }
   // Intraday::LoadData(ticker, md_path, tas_path) (intraday.cpp:141-150) on a tape Session: the CSV pair is read by
   // rlm_ingest_csv and becomes a one-day library.  The venue's tick table is the config's (the reference derives it from
   // the ticker, market.cpp:206-245); the ticker is kept for getEpisodeId-style reporting only.

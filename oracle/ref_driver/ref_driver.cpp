@@ -144,15 +144,18 @@ void usage() {
           "                  [--theta out_theta.bin] [--quiet]\n"
           "                  [--episodes N]   N training episodes on ONE Intraday + ONE Learner-equivalent (the States and the\n"
           "                                   agent are reused, LoadData + RunEpisode per episode: main.cpp:45-60, serial.cpp:72-95)\n"
-          "                  [--test-md md.csv --test-tas tas.csv --dump-test out.bin]   evaluation phase of main.cpp:216-241\n"
+          "                  [--test-md md.csv --test-tas tas.csv [--test-symbol T] --dump-test out.bin]...\n"
+          "                                   evaluation phase of main.cpp:216-244, one group per test day: ONE Intraday for\n"
+          "                                   every day, LoadData + a new Backtester per day; --test-symbol defaults to --symbol\n"
           "                  [--log-dir d]   evaluation phase writes d/profit_log.csv, d/order_log.csv (Backtester ctor) and\n"
-          "                                  d/test_stats.csv (env.writeStats, main.cpp:244)\n");
+          "                                  d/test_stats.csv (env.writeStats after the last day, main.cpp:244)\n");
 }
 
 }  // namespace
 
 int main(int argc, char** argv) {
-  string cfg, symbol = "AAL.L", md, tas, algo, dump, theta_out, test_md, test_tas, dump_test, log_dir;
+  string cfg, symbol = "AAL.L", md, tas, algo, dump, theta_out, log_dir;
+  vector<string> test_md, test_tas, test_symbol, dump_test;  // one entry per test day
   long max_steps = -1;
   int n_episodes = 1;
   bool quiet = false;
@@ -167,15 +170,19 @@ int main(int argc, char** argv) {
     else if (a == "--steps") max_steps = atol(next().c_str());
     else if (a == "--dump") dump = next();
     else if (a == "--theta") theta_out = next();
-    else if (a == "--test-md") test_md = next();
-    else if (a == "--test-tas") test_tas = next();
-    else if (a == "--dump-test") dump_test = next();
+    else if (a == "--test-md") test_md.push_back(next());
+    else if (a == "--test-tas") test_tas.push_back(next());
+    else if (a == "--test-symbol") test_symbol.push_back(next());
+    else if (a == "--dump-test") dump_test.push_back(next());
     else if (a == "--log-dir") log_dir = next();
     else if (a == "--episodes") n_episodes = atoi(next().c_str());
     else if (a == "--quiet") quiet = true;
     else { usage(); return 2; }
   }
   if (cfg.empty() || md.empty() || tas.empty()) { usage(); return 2; }
+  const size_t n_test = test_md.size();
+  if (test_tas.size() != n_test || (!dump_test.empty() && dump_test.size() != n_test) ||
+      (!test_symbol.empty() && test_symbol.size() != n_test)) { usage(); return 2; }
 
   try {
     Config c(cfg);
@@ -296,57 +303,74 @@ int main(int argc, char** argv) {
     double secs = chrono::duration<double>(t_end - t_start).count();
     if (fd) fclose(fd);
 
-    // Evaluation phase, main.cpp:216-241: greedy agent, a NEW Intraday object, Backtester::RunEpisode
-    // (Runner::RunEpisode serial.cpp:18-34 + Backtester::_step serial.cpp:121-137).
-    long test_steps = 0;
-    rlm_step_record test_last;
-    memset(&test_last, 0, sizeof(test_last));
-    if (!test_md.empty()) {
+    // Evaluation phase, main.cpp:216-244: greedy agent, ONE new Intraday object for every test day; per day LoadData,
+    // a new Backtester (Runner::RunEpisode serial.cpp:18-34 + Backtester::_step serial.cpp:121-137).  The env object
+    // keeps what Initialise does not clear (window sums, position, experiment statistics) from one day to the next.
+    struct DaySummary { long steps; rlm_step_record last; };
+    vector<DaySummary> days;
+    if (n_test > 0) {
       m->GoGreedy();
       EnvSpy env2(c);
-      env2.LoadData(symbol, test_md, test_tas);
-      if (!log_dir.empty()) {
-        // Backtester::Backtester, serial.cpp:97-119 (pattern "%v": main.cpp:254)
-        spdlog::set_pattern("%v");
-        spdlog::rotating_logger_mt("profit_log", log_dir + "/profit_log.csv", 1u << 30, 1);
-        spdlog::get("profit_log")->info("episode,step,action,position,midprice,spread,quoted_ask,quoted_bid,ask_level,bid_level,pnl_step,bandh_step");
-        spdlog::rotating_logger_mt("trade_log", log_dir + "/order_log.csv", 1u << 30, 1);
-        spdlog::get("trade_log")->info("episode,step,position,side,action,price,size,pnl");
-        env2.start_logging();
+      for (size_t day = 0; day < n_test; ++day) {
+        env2.LoadData(test_symbol.empty() ? symbol : test_symbol[day], test_md[day], test_tas[day]);
+        if (!log_dir.empty()) {
+          // Backtester::Backtester, serial.cpp:97-119 (pattern "%v": main.cpp:254).  From the second day on the
+          // loggers exist: rotating_logger_mt throws and the ctor swallows it, so the files keep one header.
+          spdlog::set_pattern("%v");
+          try {
+            spdlog::rotating_logger_mt("profit_log", log_dir + "/profit_log.csv", 1u << 30, 1);
+            spdlog::get("profit_log")->info("episode,step,action,position,midprice,spread,quoted_ask,quoted_bid,ask_level,bid_level,pnl_step,bandh_step");
+          } catch (const std::exception&) {}
+          try {
+            spdlog::rotating_logger_mt("trade_log", log_dir + "/order_log.csv", 1u << 30, 1);
+            spdlog::get("trade_log")->info("episode,step,position,side,action,price,size,pnl");
+          } catch (const std::exception&) {}
+          env2.start_logging();
+        }
+        rl::State b1(c), b2(c);  // Runner ctor, serial.cpp:9-16
+        rl::State* bstate = &b1;
+        rl::State* blast = &b2;
+        FILE* ft2 = dump_test.empty() ? nullptr : fopen(dump_test[day].c_str(), "wb");
+        if (!dump_test.empty() && !ft2) throw runtime_error("cannot open dump file " + dump_test[day]);
+        if (!env2.Initialise()) throw runtime_error("Initialise() failed on the test data");
+        blast->newState(env2);
+        long test_steps = 0;
+        while (true) {
+          if (env2.isTerminal()) break;
+          bstate->newState(env2);
+          int action = m->action(*bstate);
+          if (!env2.performAction(action)) break;
+          rlm_step_record r;
+          memset(&r, 0, sizeof(r));
+          r.step = (int32_t)test_steps;
+          r.action = action;
+          env2.fill(r);
+          r.reward = env2.getReward();
+          auto& sv = bstate->toVector();
+          r.n_state = (int32_t)sv.size();
+          for (size_t i = 0; i < sv.size() && i < RLM_N_STATE_MAX; ++i) r.state[i] = sv[i];
+          r.n_traces = av.traces()->n_nonzero_traces;
+          if (ft2) fwrite(&r, sizeof(r), 1, ft2);
+          ++test_steps;
+        }
+        env2.ClearInventory();
+        DaySummary ds;
+        ds.steps = test_steps;
+        memset(&ds.last, 0, sizeof(ds.last));
+        env2.fill(ds.last);
+        days.push_back(ds);
+        if (ft2) fclose(ft2);
       }
-      rl::State b1(c), b2(c);  // Runner ctor, serial.cpp:9-16
-      rl::State* bstate = &b1;
-      rl::State* blast = &b2;
-      FILE* ft2 = dump_test.empty() ? nullptr : fopen(dump_test.c_str(), "wb");
-      if (!env2.Initialise()) throw runtime_error("Initialise() failed on the test data");
-      blast->newState(env2);
-      while (true) {
-        if (env2.isTerminal()) break;
-        bstate->newState(env2);
-        int action = m->action(*bstate);
-        if (!env2.performAction(action)) break;
-        rlm_step_record r;
-        memset(&r, 0, sizeof(r));
-        r.step = (int32_t)test_steps;
-        r.action = action;
-        env2.fill(r);
-        r.reward = env2.getReward();
-        auto& sv = bstate->toVector();
-        r.n_state = (int32_t)sv.size();
-        for (size_t i = 0; i < sv.size() && i < RLM_N_STATE_MAX; ++i) r.state[i] = sv[i];
-        r.n_traces = av.traces()->n_nonzero_traces;
-        if (ft2) fwrite(&r, sizeof(r), 1, ft2);
-        ++test_steps;
-      }
-      env2.ClearInventory();
-      env2.fill(test_last);
       if (!log_dir.empty()) {
         spdlog::get("profit_log")->flush();
         spdlog::get("trade_log")->flush();
         env2.writeStats(log_dir + "/test_stats.csv");  // main.cpp:244
       }
-      if (ft2) fclose(ft2);
     }
+    const long test_steps = days.empty() ? 0 : days.back().steps;
+    rlm_step_record test_last;
+    memset(&test_last, 0, sizeof(test_last));
+    if (!days.empty()) test_last = days.back().last;
 
     if (!theta_out.empty()) {
       // sparse dump: (int64 index, double value) for every nonzero weight of table A
@@ -373,10 +397,21 @@ int main(int argc, char** argv) {
              steps, terminal ? 1 : 0, secs, steps / std::max(secs, 1e-12), r.time_ms, (long long)r.position,
              r.ep_pnl, r.ep_reward, sum_reward, r.ask_transactions, r.bid_transactions);
       for (unsigned a = 0; a < n_actions && a < 16; ++a) printf("%s%ld", a ? ", " : "", hist[a]);
-      printf("], \"test_steps\": %ld, \"test_position\": %lld, \"test_ep_pnl\": %.17g, \"test_ep_reward\": %.17g, "
-             "\"test_ask_tx\": %d, \"test_bid_tx\": %d, \"test_market_buys\": %d, \"test_market_sells\": %d}\n",
-             test_steps, (long long)test_last.position, test_last.ep_pnl, test_last.ep_reward, test_last.ask_transactions,
-             test_last.bid_transactions, test_last.market_buys, test_last.market_sells);
+      // one summary per test day after a multi-day evaluation; the test_* fields before it are the last day's
+      auto day_json = [](long n, const rlm_step_record& l) {
+        char buf[512];
+        snprintf(buf, sizeof(buf), "\"test_steps\": %ld, \"test_position\": %lld, \"test_ep_pnl\": %.17g, \"test_ep_reward\": %.17g, "
+                 "\"test_ask_tx\": %d, \"test_bid_tx\": %d, \"test_market_buys\": %d, \"test_market_sells\": %d",
+                 n, (long long)l.position, l.ep_pnl, l.ep_reward, l.ask_transactions, l.bid_transactions, l.market_buys, l.market_sells);
+        return string(buf);
+      };
+      printf("], %s", day_json(test_steps, test_last).c_str());
+      if (days.size() > 1) {
+        printf(", \"test_days\": [");
+        for (size_t d = 0; d < days.size(); ++d) printf("%s{%s}", d ? ", " : "", day_json(days[d].steps, days[d].last).c_str());
+        printf("]");
+      }
+      printf("}\n");
     }
     delete m;
     return 0;

@@ -595,6 +595,20 @@ int rlm_new_env(rlm_handle h, const rlm_flow_params* flow) {
   return RLM_OK;
 }
 
+int rlm_set_flow(rlm_handle h, const rlm_flow_params* flow) {
+  API_LOCK;
+  if (!h || !flow) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_set_flow: bad arguments");
+  if (h->cfg.source != RLM_SOURCE_GENERATOR)
+    return fail(RLM_ERR_INVALID_ARGUMENT, h->cfg.source == RLM_SOURCE_TAPE ? "rlm_set_flow: a tape handle changes days with rlm_assign_days"
+                                                                           : "rlm_set_flow: a stream handle loads its next day with rlm_load_ticks");
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));  // running kernels read the old parameters from constant memory
+  h->cfg.flow = *flow;
+  h->hp.flow = *flow;
+  if (g_params_owner == h) g_params_owner = nullptr;  // rlm_reset uploads them again (after a device-wide synchronisation)
+  return RLM_OK;
+}
+
 int rlm_load_ticks(rlm_handle h, const rlm_tick_msg* msgs, int32_t n_ticks) {
   API_LOCK;
   if (!h || !msgs || n_ticks <= 0) return fail(RLM_ERR_INVALID_ARGUMENT, "bad arguments");

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RLM_LIB_PATH") or os.path.join(_HERE, "librlm.so")  # (RLM_LIB_PATH: the phase-timeline build of tools/phase_probe.py)
 
 EXPORTS = [
-    "rlm_last_error", "rlm_abi_version", "rlm_config_default", "rlm_create", "rlm_destroy", "rlm_reset", "rlm_set_mode", "rlm_new_env",
+    "rlm_last_error", "rlm_abi_version", "rlm_config_default", "rlm_create", "rlm_destroy", "rlm_reset", "rlm_set_mode", "rlm_new_env", "rlm_set_flow",
     "rlm_load_ticks", "rlm_load_days", "rlm_assign_days", "rlm_get_tape_pos", "rlm_set_day_markets", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
     "rlm_get_reward", "rlm_get_actions", "rlm_get_rho", "rlm_get_occupancy", "rlm_copy_theta", "rlm_handle_terminal", "rlm_go_greedy", "rlm_read_theta",
     "rlm_write_theta", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
@@ -50,6 +50,7 @@ def load():
     L.rlm_reset.argtypes = [C.c_void_p]
     L.rlm_set_mode.argtypes = [C.c_void_p, C.c_int32]
     L.rlm_new_env.argtypes = [C.c_void_p, P(abi.FlowParams)]
+    L.rlm_set_flow.argtypes = [C.c_void_p, P(abi.FlowParams)]
     L.rlm_load_ticks.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
     L.rlm_load_days.argtypes = [C.c_void_p, C.c_void_p, P(C.c_int64), C.c_int32]
     L.rlm_assign_days.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_int32)]
@@ -151,6 +152,12 @@ class BatchedMarket:
         check(self.L.rlm_new_env(self.h, C.byref(flow) if flow is not None else None))
         if flow is not None:
             self.cfg.flow = flow
+
+    def set_flow(self, flow):
+        """LoadData of another synthetic day on the same env objects (generator source); follow with reset().  The
+        next test day of main.cpp:219-241, whose env object outlives the day (new_env is the first test day only)."""
+        check(self.L.rlm_set_flow(self.h, C.byref(flow)))
+        self.cfg.flow = flow
 
     def load_ticks(self, msgs, n_ticks):
         """msgs: ctypes array (or address) of TickMsg laid out [tick][env]; kept alive until sync()."""

@@ -170,10 +170,15 @@ def write_ref_yaml(path, ydict):
 
 
 def run_ref(ydict, flow_seed, env_index, n_ticks, dt_ms=250, max_steps=-1, algo=None, want_theta=False, t0_ms=None,
-            test=None, episodes=1):
+            test=None, episodes=1, tests=None):
     """Run the UNMODIFIED reference (oracle/_ref/ref_driver) on the CSV rendering of the same flow.
     test = dict(flow_seed, env, ticks, t0_ms): also run main.cpp's evaluation phase (greedy agent, new env,
-    Backtester) on a second stream; its records come back as "test_records"."""
+    Backtester) on a second stream; its records come back as "test_records".
+    tests = [day, ...]: main.cpp's evaluation phase over several test days on ONE env object (main.cpp:216-244); a day is
+    dict(flow_seed, env, ticks, t0_ms) for a synthetic stream or dict(md, tas) for a CSV pair, each optionally with
+    "symbol" (default: the yaml's).  The records of day d come back as "test_days"[d]; logs=True on the first day
+    collects the evaluation logs of all days."""
+    assert not (test and tests), "test= and tests= are two spellings of the evaluation phase"
     assert have_ref(), "oracle/_ref/ref_driver not built"
     with tempfile.TemporaryDirectory() as d:
         md, tas = os.path.join(d, "x_md_1.csv"), os.path.join(d, "x_tas_1.csv")
@@ -202,6 +207,23 @@ def run_ref(ydict, flow_seed, env_index, n_ticks, dt_ms=250, max_steps=-1, algo=
             if test.get("logs"):
                 os.makedirs(os.path.join(d, "logs"))
                 cmd += ["--log-dir", os.path.join(d, "logs")]
+        day_dumps = []
+        for k, t in enumerate(tests or []):
+            if "md" in t:
+                mdk, task = t["md"], t["tas"]
+            else:
+                mdk, task = os.path.join(d, "t%d_md_1.csv" % k), os.path.join(d, "t%d_tas_1.csv" % k)
+                t0k = [] if t.get("t0_ms") is None else ["--t0-ms", str(t["t0_ms"])]
+                subprocess.check_call([FLOW_CSV, "--seed", str(t["flow_seed"]), "--env", str(t["env"]), "--ticks", str(t["ticks"]),
+                                       "--dt-ms", str(dt_ms), "--md", mdk, "--tas", task] + t0k)
+            day_dumps.append(os.path.join(d, "test_steps_%d.bin" % k))
+            cmd += ["--test-md", mdk, "--test-tas", task, "--dump-test", day_dumps[-1]]
+            if t.get("symbol"):
+                cmd += ["--test-symbol", t["symbol"]]
+        want_logs = bool((test or {}).get("logs") or (tests and tests[0].get("logs")))
+        if tests and want_logs:
+            os.makedirs(os.path.join(d, "logs"))
+            cmd += ["--log-dir", os.path.join(d, "logs")]
         out = subprocess.check_output(cmd)
         summary = json.loads(out.decode().strip().splitlines()[-1])
         raw = open(dump, "rb").read()
@@ -216,12 +238,19 @@ def run_ref(ydict, flow_seed, env_index, n_ticks, dt_ms=250, max_steps=-1, algo=
                 idx, val = struct.unpack("<qd", tr[i:i + 16])
                 theta[idx] = val
         test_records, logs = None, None
-        if test and test.get("logs"):
+        if want_logs:
             logs = {n: open(os.path.join(d, "logs", n)).read() for n in ("profit_log.csv", "test_stats.csv", "order_log.csv")}
+        test_days = [_read_records(p) for p in day_dumps] if tests else None
         if test:
             raw2 = open(dump2, "rb").read()
             n2 = len(raw2) // C.sizeof(abi.StepRecord)
             recs2 = (abi.StepRecord * n2).from_buffer_copy(raw2)
             test_records = [recs2[i] for i in range(n2)]
     return {"records": [recs[i] for i in range(n)], "summary": summary, "theta": theta, "_keep": recs,
-            "test_records": test_records, "logs": logs}
+            "test_records": test_records, "logs": logs, "test_days": test_days}
+
+
+def _read_records(path):
+    raw = open(path, "rb").read()
+    arr = (abi.StepRecord * (len(raw) // C.sizeof(abi.StepRecord))).from_buffer_copy(raw)
+    return [arr[i] for i in range(len(arr))]

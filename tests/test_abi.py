@@ -109,6 +109,19 @@ def test_no_cpu_fallback():
     assert lib.load().rlm_test_to_ticks(C.byref(cfg), px, 1, out) == abi.RLM_ERR_NO_DEVICE
 
 
+def test_set_flow_binding_and_argument_checks():
+    """rlm_set_flow (LoadData of another synthetic day on the same env objects) is bound with the header's types and
+    refuses a missing handle or flow before it touches a device; the ABI version is unchanged by the addition."""
+    L = lib.load()
+    assert L.rlm_set_flow.argtypes == [C.c_void_p, C.POINTER(abi.FlowParams)]
+    assert L.rlm_abi_version() == 4
+    flow = config.from_dict(config.example_dict(), flow_seed=5).flow
+    assert L.rlm_set_flow(None, C.byref(flow)) == abi.RLM_ERR_INVALID_ARGUMENT
+    assert "rlm_set_flow" in L.rlm_last_error().decode()
+    assert L.rlm_set_flow(None, None) == abi.RLM_ERR_INVALID_ARGUMENT
+    assert hasattr(lib.BatchedMarket, "set_flow")
+
+
 def test_product_does_not_import_the_oracle():
     for root, _dirs, files in os.walk(os.path.join(ROOT, "rl_markets_b200")):
         for f in files:

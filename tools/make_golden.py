@@ -3,6 +3,8 @@
 the reference sources are present, see oracle/Makefile; the fixtures are committed so that
 machines without the reference can check against them).
   --reference-checks   only the fixtures of reference_checks() below
+  --day-markets        only tests/golden/day_markets.json and its digests (day_market_fixtures())
+  --eval-days          only tests/golden/eval_days.json and its digests (eval_days_fixtures())
 
   tests/golden/units.json          reference unit-level vectors (oracle/_ref/ref_units)
   tests/golden/steps_<name>.bin    first N rlm_step_record of a reference run (oracle/_ref/ref_driver)
@@ -276,10 +278,9 @@ def main():
     reference_checks()
 
 
-def _keep_wall_clock(manifest):
+def _keep_wall_clock(manifest, path=os.path.join(GOLD, "manifest.json")):
     """The reference's run time is in the summaries it printed; an entry whose outputs did not change keeps the stored
-    time, so that regenerating leaves manifest.json as it was."""
-    path = os.path.join(GOLD, "manifest.json")
+    time, so that regenerating leaves the fixture file (manifest.json, eval_days.json) as it was."""
     if not os.path.exists(path):
         return
     old = {c["name"]: c for c in json.load(open(path))}
@@ -373,10 +374,93 @@ def day_market_fixtures():
         json.dump(dict(yaml=y, env0=DAY_MARKETS_ENV0, days=days), f, indent=1)
 
 
+# Evaluation over several test days (main.cpp:216-244): train until the close, GoGreedy, then ONE Intraday object for
+# every test day -- LoadData, a new Backtester, Initialise, the steps, ClearInventory.  What Initialise leaves alone
+# (the window sums of Accumulator::clear and RollingMean, A13; position; the greedy agent's rand()) runs from one day
+# into the next.  A day is a synthetic stream (flow_seed, ticks, open_ticks; env = the case's) or a venue day
+# (venue = a VENUE_CASES name, under its ticker's market).  Written to tests/golden/eval_days.json and
+# digests_ed_<case>_{train,day<d>}.bin, not into manifest.json.
+def _ed(name, algo, M, env, flow_seed, over, n_days=3, days=None):
+    days = days or [dict(flow_seed=flow_seed + 1 + d, ticks=1000, open_ticks=700) for d in range(n_days)]
+    return dict(name=name, algo=algo, M=M, env=env, flow_seed=flow_seed, ticks=1200, train_open_ticks=900, over=over, days=days)
+
+
+_VARS4 = ["pos", "spd", "vol", "svl"]
+EVAL_DAYS_CASES = [
+    _ed("ed_double_q_default", "double_q_learn", 8192, 70, 201, {"learning.alpha_start": 0.01}),
+    _ed("ed_q_vars13_micro_m5003", "q_learn", 5003, 71, 205,
+        {"state.variables": _ALL_VARS, "state.lookback.rsi": 10, "state.lookback.vwap": 20,
+         "market.target_price.type": "microprice", "market.target_price.lookback": 5}),
+    _ed("ed_sarsa", "sarsa", 8192, 72, 209, {}, n_days=2),
+    _ed("ed_r_learn", "r_learn", 8192, 73, 213, {"policy.eps_init": 0.3}, n_days=2),
+    _ed("ed_online_r_learn", "online_r_learn", 8192, 74, 217, {"policy.eps_init": 0.3}, n_days=2),
+    _ed("ed_double_r_learn", "double_r_learn", 8209, 75, 221, {"policy.eps_init": 0.3, "learning.alpha_start": 0.01}, n_days=2),
+    _ed("ed_act5_vars4", "q_learn", 8192, 76, 225, {"learning.n_actions": 5, "state.variables": _VARS4}),
+    _ed("ed_tickers_aal_baes", "q_learn", 8192, 77, 229, {}, days=[dict(venue="venue_aal_l"), dict(venue="venue_baes_l")]),
+]
+
+
+def eval_days_yaml(c):
+    return config.example_dict(**{"learning.memory_size": c["M"], "learning.algorithm": c["algo"], **c["over"]})
+
+
+def eval_day_inputs(c, d):
+    """The days of case c as ol.run_ref takes them (venue days written as CSV pairs into directory d), and the same
+    days with their t0_ms / ticker filled in for the fixture."""
+    import golden_util
+    cfg = config.from_dict(eval_days_yaml(c))
+    venues = {v["name"]: v for v in VENUE_CASES}
+    runs, days = [], []
+    for k, day in enumerate(c["days"]):
+        if "venue" in day:
+            v = venues[day["venue"]]
+            sub = os.path.join(d, "day%d" % k)
+            os.makedirs(sub)
+            md, tas = golden_util.venue_day(v, sub)
+            runs.append(dict(md=md, tas=tas, symbol=v["ticker"]))
+            days.append(dict(day, ticker=v["ticker"], md_sha256=file_sha256(md), tas_sha256=file_sha256(tas)))
+        else:
+            t = dict(day, env=c["env"], t0_ms=day_t0(cfg, day["open_ticks"]))
+            runs.append(t)
+            days.append(t)
+    return runs, days
+
+
+def eval_days_fixtures():
+    import tempfile
+    import hashlib
+    out = []
+    for c in EVAL_DAYS_CASES:
+        y = eval_days_yaml(c)
+        y_run = json.loads(json.dumps(y))
+        y_run["debug"]["random_seed"] = y["debug"]["random_seed"] + c["env"]
+        t0 = day_t0(config.from_dict(y), c["train_open_ticks"])
+        with tempfile.TemporaryDirectory() as d:
+            runs, days = eval_day_inputs(c, d)
+            runs[0] = dict(runs[0], logs=True)
+            ref = ol.run_ref(y_run, c["flow_seed"], c["env"], c["ticks"], t0_ms=t0, tests=runs)
+        assert ref["summary"]["terminal"] == 1
+        _write_digests(c["name"] + "_train", ref["records"])
+        per_day = ref["summary"]["test_days"]
+        for k, recs in enumerate(ref["test_days"]):
+            assert len(recs) == per_day[k]["test_steps"] > 100, (c["name"], k, len(recs))
+            _write_digests("%s_day%d" % (c["name"], k), recs)
+            days[k] = dict(days[k], n_records=len(recs), summary=per_day[k])
+        logs = {n: hashlib.sha256(ref["logs"][n].encode()).hexdigest() for n in ("profit_log.csv", "test_stats.csv")}
+        out.append(dict(c, yaml=y, t0_ms=t0, days=days, n_records=len(ref["records"]), logs_sha256=logs,
+                        summary={k: v for k, v in ref["summary"].items() if k != "test_days"}))
+    path = os.path.join(GOLD, "eval_days.json")
+    _keep_wall_clock(out, path)
+    with open(path, "w") as f:
+        json.dump(out, f, indent=1)
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["--reference-checks"]:
         reference_checks()
     elif sys.argv[1:] == ["--day-markets"]:
         day_market_fixtures()
+    elif sys.argv[1:] == ["--eval-days"]:
+        eval_days_fixtures()
     else:
         main()
