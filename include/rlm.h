@@ -302,7 +302,25 @@ int rlm_apply_dtheta(rlm_handle h);
  * actions_out[b] / the action applied is -1 for an env whose episode is over or whose tape day has run out.
  * terminal_out[b]: 1 = the episode is over (Intraday::isTerminal), 2 = tape source: the env needed a message past the end
  * of its day and stopped inside performAction (the reference's performAction returning false at the end of its files).  rlm_env_step(h, actions != NULL) without a preceding rlm_act
- * is the "external policy" form: no generator draw is consumed.  Independent policies only. */
+ * is the "external policy" form: no generator draw is consumed.
+ *
+ * In RLM_MODE_TRAIN (above) the calls are Learner::_step, for independent policies only (a shared_policy handle trains
+ * with rlm_shared_tick_accumulate / rlm_apply_dtheta: RLM_ERR_UNSUPPORTED here).  In RLM_MODE_BACKTEST they are
+ * experiment::serial::Backtester::_step (serial.cpp:124-137), for independent and shared policies alike:
+ *
+ *   rlm_env_step(h, NULL, ..)        Runner::RunEpisode: environment.Initialise()              serial.cpp:21-22
+ *   rlm_agent_update(h, NULL)        last_state->newState(environment): the first decision state serial.cpp:25
+ *   repeat:
+ *     rlm_act(h, actions)            int action = m->action(*state)  (-1: isTerminal, the day is over) serial.cpp:131
+ *     rlm_env_step(h, actions, r, t) environment.performAction(action)                         serial.cpp:133
+ *     rlm_agent_update(h, delta)     state->newState(environment) of the next _step            serial.cpp:129
+ *
+ * rlm_agent_update runs the greedy evaluation step on the envs whose step ended: it reads theta of the env's policy (policy
+ * 0 on a shared handle) and never writes theta, dtheta or the traces; delta_out gets 0.0 for every env.  Driven in this
+ * order the calls reproduce rlm_run_ticks in backtest mode bit for bit (records, rlm_env_stats, counters, day-market
+ * terminal flags), and rlm_run_ticks continues every env where they left it.  With external actions (rlm_env_step without
+ * rlm_act) the records carry the caller's actions and every profit_log column, and rlm_get_stats the counters of
+ * Base::writeStats: a caller's own quoting policy backtested under the reference's P&L accounting. */
 int rlm_act(rlm_handle h, int32_t* actions_out /* [n_envs] */);
 int rlm_env_step(rlm_handle h, const int32_t* actions /* [n_envs] or NULL = the agent's own */, double* reward_out /* [n_envs] or NULL */,
                  uint8_t* terminal_out /* [n_envs] or NULL */);

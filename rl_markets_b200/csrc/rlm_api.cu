@@ -1409,13 +1409,16 @@ int rlm_apply_dtheta(rlm_handle h) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// Split surface: the reference's Environment::step / Agent::update seam (SURVEY.md 8b), batched.
+// Split surface: the reference's Environment::step / Agent::update seam (SURVEY.md 8b), batched.  In train mode the three
+// calls are Learner::_step, in backtest mode Backtester::_step: the same tick kernels, with the evaluation kernel in the
+// learner's place (launch_agent_on), which only reads theta -- so a shared handle may evaluate here, but not train.
 static int split_check(rlm_handle h) {
   if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
-  if (h->cfg.shared_policy) return fail(RLM_ERR_UNSUPPORTED, "the split surface drives independent policies (shared policy: rlm_shared_tick_accumulate / rlm_apply_dtheta)");
   if (h->cfg.source == RLM_SOURCE_STREAM)
     return fail(RLM_ERR_UNSUPPORTED, "the split surface needs source = generator or tape: envs consume different numbers of ticks per step");
-  if (h->dyn.backtest) return fail(RLM_ERR_UNSUPPORTED, "the split surface runs Learner::_step (train mode)");
+  if (h->cfg.shared_policy && !h->dyn.backtest)
+    return fail(RLM_ERR_UNSUPPORTED, "the split surface trains independent policies only (shared-policy training: rlm_shared_tick_accumulate / "
+                                     "rlm_apply_dtheta; a shared handle in backtest mode may use the split surface)");
   return tape_check(h);
 }
 static DynParams split_dyn(rlm_handle h) {
@@ -1496,11 +1499,15 @@ int rlm_agent_update(rlm_handle h, double* delta_out) {
   rc = upload_params(h);
   if (rc) return rc;
   const int B = h->cfg.n_envs;
-  // State::newState + Agent::HandleTransition for the envs on the ready list of the last rlm_env_step
+  // State::newState + Agent::HandleTransition for the envs on the ready list of the last rlm_env_step (backtest mode:
+  // State::newState of the next Backtester::_step, the greedy evaluation step)
   CK(launch_agent_any(h, split_dyn(h), 0, 0));
   CK(cudaMemsetAsync(h->ptr.ready_count, 0, 4, h->stream));
   h->launches += 1;
-  if (delta_out) {
+  if (delta_out && h->dyn.backtest) {
+    // Backtester::_step computes no TD error (AgentD::last_delta may still hold the last one of training)
+    memset(delta_out, 0, (size_t)B * 8);
+  } else if (delta_out) {
     rc = split_scratch(h, (size_t)B * 8);
     if (rc) return rc;
     CK(rlm_launch_step_out(h->ptr, B, nullptr, nullptr, (double*)h->d_gather, h->stream));

@@ -284,23 +284,28 @@ class BatchedMarket:
         check(self.L.rlm_get_kernel_times(self.h, C.byref(a), C.byref(b), C.byref(na), C.byref(nb)))
         return {"env_ms": a.value, "agent_ms": b.value, "env_launches": na.value, "agent_launches": nb.value}
 
-    # ---- split surface: Environment::step / Agent::update (include/rlm.h)
+    # ---- split surface: Environment::step / Agent::update (include/rlm.h).  Train mode: Learner::_step (independent
+    # policies); backtest mode: Backtester::_step (independent and shared policies)
     def act(self):
-        """Agent::action for every env at a decision point (-1 elsewhere)."""
+        """Agent::action for every env at a decision point (-1 elsewhere, and where the episode is over).  Backtest mode:
+        the greedy action from the state the last agent_update built."""
         out = (C.c_int32 * self.cfg.n_envs)()
         check(self.L.rlm_act(self.h, out))
         return out
 
     def env_step(self, actions=None):
         """Base::performAction + getReward: one learner step's worth of ticks per env.  Returns (rewards, terminal):
-        terminal[b] is 1 when env b's episode is over, 2 when its tape day ran out inside performAction (tape source)."""
+        terminal[b] is 1 when env b's episode is over, 2 when its tape day ran out inside performAction (tape source).
+        actions given without act(): the caller's own actions (no policy draw), in either mode."""
         n = self.cfg.n_envs
         rew, term = (C.c_double * n)(), (C.c_uint8 * n)()
         check(self.L.rlm_env_step(self.h, actions, rew, term))
         return rew, term
 
     def agent_update(self):
-        """State::newState + Agent::HandleTransition for the envs whose step ended; returns the TD errors."""
+        """Train mode: State::newState + Agent::HandleTransition for the envs whose step ended; returns the TD errors.
+        Backtest mode: State::newState of the next Backtester::_step (the greedy evaluation step; theta is only read);
+        returns zeros, Backtester::_step computes no TD error."""
         out = (C.c_double * self.cfg.n_envs)()
         check(self.L.rlm_agent_update(self.h, out))
         return out
