@@ -23,6 +23,7 @@
  *   rlm_handle_terminal   Agent::HandleTerminal + Policy::HandleTerminal   src/rl/agent.cpp:103-109, policy.cpp:79-82
  *   rlm_go_greedy         Agent::GoGreedy                                  src/rl/agent.cpp:76-79
  *   rlm_read_theta        Agent::write_theta (raw double[MEMORY_SIZE])     src/rl/agent.cpp:176-181
+ *   rlm_eval_q            Agent::getQ / DoubleAgent::getQb on any states   src/rl/agent.cpp:117-135,211-230
  *   rlm_get_stats         Base::getEpisodeReward/getEpisodePnL/...         src/environment/base.cpp:244-252,458-473
  *
  * Conventions: plain C types only; every call returns 0 on success or a
@@ -267,6 +268,24 @@ int rlm_go_greedy(rlm_handle h);
 /* theta access: policy = env index (independent) or 0 (shared); table 0 = A, 1 = B (double agents). */
 int rlm_read_theta(rlm_handle h, int32_t policy, int32_t table, double* out, int64_t n);
 int rlm_write_theta(rlm_handle h, int32_t policy, int32_t table, const double* in, int64_t n);
+
+/* Agent::getQ / DoubleAgent::getQb (agent.cpp:117-135, 211-230) on State::newState(vars, .) (state.cpp:45-51).
+ * q_out[i][t][a]: query i, table t (0 = A: getQ; 1 = B: getQb, double_q_learn / double_r_learn only), action a < n_actions.
+ * - vars != NULL: query i is tile-coded from vars[i] exactly as tiles() does it (NaN and out-of-range values included:
+ *   x86's truncation) and evaluated under the theta of policy[i] (policy == NULL: policy 0).  Independent handles take
+ *   0 <= policy[i] < n_envs, shared handles NULL or all zeros.
+ * - vars == NULL, the live form: n == n_envs and policy == NULL.  Row b is Q of env b's current decision state (the one
+ *   rlm_get_state returns for b; before the first newState the never-populated State, every feature index 0, as the
+ *   learner treats it) under env b's own policy (policy 0 on a shared handle).  Between rlm_agent_update and rlm_act these
+ *   rows are what Agent::action samples from; a double agent samples (Q_A + Q_B) / 2.0, one IEEE operation on the host.
+ * The call only reads theta: theta, dtheta, traces, agent state, generators, records, statistics and counters stay as
+ * they were, in both modes and for every algorithm, source and engine.  It runs on the handle's stream after the work
+ * already enqueued and returns when q_out is filled; queries go through device scratch in chunks of RLM_EVAL_Q_CHUNK, so
+ * device memory does not grow with n.  A null handle or q_out, n < 0, a policy index out of range, or a live-form call
+ * with n != n_envs or policy != NULL return RLM_ERR_INVALID_ARGUMENT with q_out untouched; n == 0 does nothing. */
+#define RLM_EVAL_Q_CHUNK (1 << 17)
+int rlm_eval_q(rlm_handle h, const float* vars /* [n][n_state_vars] or NULL */, const int32_t* policy /* [n] or NULL */,
+               int64_t n, double* q_out /* [n][n_tables][n_actions] */);
 
 /* parity dump of recorded envs (cfg.record_envs / record_cap) */
 int rlm_read_records(rlm_handle h, int32_t env, rlm_step_record* out, int32_t cap, int32_t* n_out);

@@ -149,8 +149,22 @@ class Agent {
     out.resize((size_t)s_.config().memory_size);
     check(rlm_read_theta(s_.handle(), 0, 0, out.data(), (int64_t)out.size()));
   }
+  // Agent::getQ (agent.cpp:117-135) and DoubleAgent::getQb (:211-230) with State::newState(vars, .) (state.cpp:45-51) folded
+  // in: the State objects live in the Session, so the state comes as its variables.  getQb needs a double agent.
+  double getQ(const std::vector<float>& vars, int action) const { return q(vars, action, 0); }
+  double getQb(const std::vector<float>& vars, int action) const { return q(vars, action, 1); }
 
  private:
+  double q(const std::vector<float>& vars, int action, int table) const {
+    const rlm_config& c = s_.config();
+    const int T = (c.algorithm == RLM_ALGO_DOUBLE_Q_LEARN || c.algorithm == RLM_ALGO_DOUBLE_R_LEARN) ? 2 : 1;
+    if ((int)vars.size() != c.n_state_vars) throw std::invalid_argument("Agent::getQ: vars must hold n_state_vars values");
+    if (action < 0 || action >= c.n_actions) throw std::invalid_argument("Agent::getQ: action out of range");
+    if (table >= T) throw std::invalid_argument("Agent::getQb: the agent has one table (not a double agent)");
+    double out[2 * RLM_MAX_ACTIONS];
+    check(rlm_eval_q(s_.handle(), vars.data(), nullptr, 1, out));
+    return out[table * c.n_actions + action];
+  }
   Session& s_;
 };
 

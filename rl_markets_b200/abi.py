@@ -12,6 +12,7 @@ RLM_N_STATE_MAX = 13
 RLM_MAX_BANDS = 32
 RLM_MAX_ACTIONS = 9
 RLM_N_TILINGS = 32
+RLM_EVAL_Q_CHUNK = 1 << 17  # queries per device pass of rlm_eval_q
 
 # enums (include/rlm.h)
 ALGO = {"q_learn": 0, "sarsa": 1, "double_q_learn": 2, "r_learn": 3, "online_r_learn": 4, "double_r_learn": 5}

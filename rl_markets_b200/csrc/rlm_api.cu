@@ -1311,6 +1311,55 @@ int rlm_write_theta(rlm_handle h, int32_t policy, int32_t table, const double* i
   return RLM_OK;
 }
 
+// Agent::getQ / DoubleAgent::getQb on State::newState(vars, .) for a batch of states (rlm_q_kernel).  Every argument is
+// checked before anything is launched or written; the queries then go through the handle's staging area in chunks of
+// RLM_EVAL_Q_CHUNK, so device memory does not grow with n.  Only theta and the env headers' decision states are read.
+int rlm_eval_q(rlm_handle h, const float* vars, const int32_t* policy, int64_t n, double* q_out) {
+  API_LOCK;
+  if (!h || !q_out) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_eval_q: null handle or q_out");
+  if (n < 0) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_eval_q: n < 0");
+  if (!vars) {
+    if (policy) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_eval_q: the live form (vars == NULL) evaluates each env under its own policy: policy must be NULL");
+    if (n != h->cfg.n_envs) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_eval_q: the live form (vars == NULL) needs n == n_envs");
+  } else if (policy) {
+    for (int64_t i = 0; i < n; ++i)
+      if (policy[i] < 0 || policy[i] >= h->n_policies)
+        return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_eval_q: policy[" + std::to_string(i) + "] = " + std::to_string(policy[i]) +
+                                                  " out of range (" + std::to_string(h->n_policies) + " policies)");
+  }
+  if (n == 0) return RLM_OK;
+  CK(cudaSetDevice(h->cfg.device));
+  int rc = upload_params(h);
+  if (rc) return rc;
+  const int64_t T = h->hp.is_double ? 2 : 1, A = h->cfg.n_actions, nv = h->cfg.n_state_vars;
+  const int64_t chunk = std::min<int64_t>(n, RLM_EVAL_Q_CHUNK);
+  const size_t out_b = (size_t)(chunk * T * A * 8), var_b = vars ? (size_t)(chunk * nv * 4) : 0, pol_b = policy ? (size_t)chunk * 4 : 0;
+  rc = split_scratch(h, out_b + var_b + pol_b);
+  if (rc) return rc;
+  unsigned char* d = (unsigned char*)h->d_gather;
+  unsigned char* hs = (unsigned char*)h->h_gather;
+  for (int64_t i0 = 0; i0 < n; i0 += chunk) {
+    const int64_t m = std::min(chunk, n - i0);
+    const float* dv = nullptr;
+    const int* dp = nullptr;
+    if (vars) {
+      memcpy(hs + out_b, vars + i0 * nv, (size_t)(m * nv * 4));
+      CK(cudaMemcpyAsync(d + out_b, hs + out_b, (size_t)(m * nv * 4), cudaMemcpyHostToDevice, h->stream));
+      dv = (const float*)(d + out_b);
+    }
+    if (policy) {
+      memcpy(hs + out_b + var_b, policy + i0, (size_t)m * 4);
+      CK(cudaMemcpyAsync(d + out_b + var_b, hs + out_b + var_b, (size_t)m * 4, cudaMemcpyHostToDevice, h->stream));
+      dp = (const int*)(d + out_b + var_b);
+    }
+    CK(rlm_launch_q(h->ptr, dv, dp, vars ? 0 : (int)i0, (int)m, (double*)d, h->hp.is_double, h->n_sms, h->stream));
+    CK(cudaMemcpyAsync(hs, d, (size_t)(m * T * A * 8), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    memcpy(q_out + i0 * T * A, hs, (size_t)(m * T * A * 8));
+  }
+  return RLM_OK;
+}
+
 int rlm_copy_theta(rlm_handle dst, rlm_handle src) {
   API_LOCK;
   if (!dst || !src) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");

@@ -15,6 +15,7 @@ cudaError_t rlm_launch_agent3(const DevPtrs& ptr, const DynParams& D, int n_envs
 cudaError_t rlm_launch_learn(const DevPtrs& ptr, const DynParams& D, int n_envs, int is_double, int tslot, int n_sms, int stage, int expected_steps, cudaStream_t st);
 cudaError_t rlm_launch_learn_staged(const DevPtrs& ptr, const DynParams& D, int n_envs, long long memory_size, int tslot, int n_sms, cudaStream_t st);
 cudaError_t rlm_launch_eval(const DevPtrs& ptr, const DynParams& D, int n_envs, int is_double, int tslot, int n_sms, cudaStream_t st);
+cudaError_t rlm_launch_q(const DevPtrs& ptr, const float* vars, const int* pol, int env0, int n, double* out, int is_double, int n_sms, cudaStream_t st);
 cudaError_t rlm_launch_fused2(const DevPtrs& ptr, const DynParams& D, int n_envs, int is_double, cudaStream_t st);
 cudaError_t rlm_launch_apply_dtheta(double* theta, double* dtheta, long long n, int n_sms, cudaStream_t st);
 size_t rlm_fused_smem_bytes(int is_double);

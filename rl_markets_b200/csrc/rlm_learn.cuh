@@ -706,6 +706,81 @@ cudaError_t rlm_launch_eval(const DevPtrs& ptr, const DynParams& D, int n_envs, 
 }
 
 // ---------------------------------------------------------------------------------------------
+// Q-value query (rlm_eval_q): Agent::getQ / DoubleAgent::getQb (agent.cpp:117-135,211-230) on State::newState(vars, .)
+// (state.cpp:45-51), one warp per query.  The middle of rlm_eval_kernel without the agent block: hash, 27 (54) gathers in
+// flight per lane, exact-order sums.  Nothing but `out` is written.
+//   vars != NULL: query k is vars[k][0..n_state_vars) under the theta of policy pol[k] (pol == NULL: policy 0)
+//   vars == NULL: query k is env env0 + k's decision state (AgentD::from_vars; the never-populated State while null_from)
+//                 under that env's own policy (policy 0 on a shared handle)
+// out[k][t][a]: t = 0 table A, t = 1 table B (double agents).  Per warp: the V table only, 7 KB (Double-Q 14 KB).
+#define QV_WARPS 4  // queries (warps) per CTA
+template <bool DBL>
+__global__ void __launch_bounds__(QV_WARPS * 32, EvCfg<DBL>::min_ctas) rlm_q_kernel(DevPtrs ptr, const float* vars, const int* pol, int env0, int n,
+                                                                                     double* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double* V = (double*)(smem + (size_t)warp * ln_v_bytes(DBL ? 1 : 0));
+  // (see rlm_learn_kernel: the hashing table, pulled into L1 before the first hash reads it at random)
+  for (int i = threadIdx.x; i < 64; i += QV_WARPS * 32) asm volatile("prefetch.global.L1 [%0];" ::"l"(rlm_rndseq_table + i * 32));
+  const int A = P.n_actions, T = DBL ? 2 : 1;
+  const int C = gridDim.x;  // query k -> warp (k / C) of CTA (k % C), as rlm_eval_kernel spreads its ready list
+#pragma unroll 1
+  for (int k = warp * C + blockIdx.x; k < n; k += QV_WARPS * C) {
+    const float* v;
+    bool null_state = false;
+    size_t p;
+    if (vars) {
+      v = vars + (size_t)k * P.n_state_vars;
+      p = pol ? (size_t)pol[k] : 0;
+    } else {
+      const EnvHdr* g = (const EnvHdr*)(ptr.env + (size_t)(env0 + k) * P.env_stride);
+      v = g->ag.from_vars;
+      null_state = g->ag.null_from != 0;
+      p = P.shared_policy ? 0 : (size_t)(env0 + k);
+    }
+    const LnSums h = ln_hash(rlm_rndseq_table, v, null_state, lane);
+    {
+      double va[3 * RLM_MAX_ACTIONS];
+      ln_gather_issue<0, 27>(ptr.theta + p * (size_t)P.memory_size, h, va);
+      if (DBL) {  // both tables' 54 gathers in flight together
+        double vb[3 * RLM_MAX_ACTIONS];
+        ln_gather_issue<0, 27>(ptr.theta_b + p * (size_t)P.memory_size, h, vb);
+        ln_gather_store<0, 27>(vb, lane, V + RLM_MAX_ACTIONS * LN_VROW);
+      }
+      ln_gather_store<0, 27>(va, lane, V);
+    }
+    __syncwarp();
+    const double q = ln_sums(V, DBL, lane);
+    const int a = lane & 15, t = lane >> 4;
+    if (a < A && t < T) out[((size_t)k * T + t) * A + a] = q;
+    __syncwarp();  // (every lane is done with V before the next query's weights are stored over it)
+  }
+}
+
+cudaError_t rlm_launch_q(const DevPtrs& ptr, const float* vars, const int* pol, int env0, int n, double* out, int is_double, int n_sms, cudaStream_t st) {
+  const int k = is_double ? 1 : 0;
+  const size_t smem = QV_WARPS * ln_v_bytes(is_double);
+  static int per_sm[2] = {0, 0};  // resident CTAs per SM
+  if (!per_sm[k]) {
+    cudaError_t e = is_double ? cudaFuncSetAttribute(rlm_q_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                              : cudaFuncSetAttribute(rlm_q_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    if (is_double) cudaFuncSetAttribute(rlm_q_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, RLM_SMEM_CARVEOUT);
+    else cudaFuncSetAttribute(rlm_q_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, RLM_SMEM_CARVEOUT);
+    int c = 0;
+    e = is_double ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, rlm_q_kernel<true>, QV_WARPS * 32, smem)
+                  : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, rlm_q_kernel<false>, QV_WARPS * 32, smem);
+    per_sm[k] = (e == cudaSuccess && c > 0) ? c : 1;
+  }
+  if (n <= 0) return cudaSuccess;
+  // one resident wave at most; the grid-stride loop takes the rest
+  const int grid = std::min((n + QV_WARPS - 1) / QV_WARPS, n_sms * per_sm[k]);
+  if (is_double) rlm_q_kernel<true><<<grid, QV_WARPS * 32, smem, st>>>(ptr, vars, pol, env0, n, out);
+  else rlm_q_kernel<false><<<grid, QV_WARPS * 32, smem, st>>>(ptr, vars, pol, env0, n, out);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------
 // Fused persistent engine (the default for independent-policy training): ONE launch per rlm_run_ticks call, one warp
 // per env for all `n_ticks` ticks.  The env record stays in shared memory for the whole launch; the warp runs the market
 // tick (envw_tick) and, whenever its env's midprice has moved, the learner step (ln_step) and the next action selection

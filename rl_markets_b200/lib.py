@@ -16,7 +16,7 @@ EXPORTS = [
     "rlm_last_error", "rlm_abi_version", "rlm_config_default", "rlm_create", "rlm_destroy", "rlm_reset", "rlm_set_mode", "rlm_new_env", "rlm_set_flow",
     "rlm_load_ticks", "rlm_load_days", "rlm_assign_days", "rlm_get_tape_pos", "rlm_set_day_markets", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
     "rlm_get_reward", "rlm_get_actions", "rlm_get_rho", "rlm_get_occupancy", "rlm_copy_theta", "rlm_handle_terminal", "rlm_go_greedy", "rlm_read_theta",
-    "rlm_write_theta", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
+    "rlm_write_theta", "rlm_eval_q", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
     "rlm_set_stream", "rlm_set_profiling", "rlm_get_kernel_times", "rlm_act", "rlm_env_step", "rlm_agent_update", "rlm_ingest_csv",
     "rlm_flow_generate", "rlm_test_to_ticks", "rlm_test_to_price", "rlm_test_tiles", "rlm_test_learner_tiles", "rlm_test_order",
     "rlm_test_rolling_mean",
@@ -70,6 +70,7 @@ def load():
     L.rlm_go_greedy.argtypes = [C.c_void_p]
     L.rlm_read_theta.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), C.c_int64]
     L.rlm_write_theta.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), C.c_int64]
+    L.rlm_eval_q.argtypes = [C.c_void_p, P(C.c_float), P(C.c_int32), C.c_int64, P(C.c_double)]
     L.rlm_read_records.argtypes = [C.c_void_p, C.c_int32, P(abi.StepRecord), C.c_int32, P(C.c_int32)]
     L.rlm_device_ptrs.argtypes = [C.c_void_p, P(C.c_void_p), P(C.c_void_p), P(C.c_int64)]
     L.rlm_apply_dtheta.argtypes = [C.c_void_p]
@@ -275,6 +276,43 @@ class BatchedMarket:
         buf = values if isinstance(values, C.Array) and values._type_ is C.c_double else (C.c_double * n).from_buffer_copy(bytes(values))
         assert len(buf) == n, (len(buf), n)
         check(self.L.rlm_write_theta(self.h, policy, table, buf, n))
+
+    @property
+    def n_tables(self):
+        return 2 if self.cfg.algorithm in (abi.ALGO["double_q_learn"], abi.ALGO["double_r_learn"]) else 1
+
+    def q_values(self, vars=None, policy=None):
+        """Agent::getQ / DoubleAgent::getQb (rlm_eval_q) -> float64 array [n][n_tables][n_actions]; [:, 1] is Q_B.
+
+        vars: float32 array [n][n_state_vars], tile-coded as State::newState(vars, .) does, each row under the theta of
+        policy[i] (int32 [n]; None = policy 0).  vars=None: the live form, Q of every env's current decision state under its
+        own policy (the values Agent::action samples from between agent_update and act).  The call only reads theta."""
+        import numpy as np
+        T, A, nv = self.n_tables, self.cfg.n_actions, self.cfg.n_state_vars
+        if vars is None:
+            if policy is not None:
+                raise ValueError("q_values: the live form (vars=None) evaluates each env under its own policy; policy must be None")
+            n, vp = self.cfg.n_envs, None
+        else:
+            vars = np.asarray(vars)
+            if vars.dtype != np.float32:
+                raise TypeError("q_values: vars must be float32, got %s" % vars.dtype)
+            if vars.ndim != 2 or vars.shape[1] != nv:
+                raise ValueError("q_values: vars must have shape (n, %d), got %s" % (nv, vars.shape))
+            vars = np.ascontiguousarray(vars)
+            n, vp = vars.shape[0], vars.ctypes.data_as(C.POINTER(C.c_float))
+        pp = None
+        if policy is not None:
+            policy = np.asarray(policy)
+            if policy.dtype != np.int32:
+                raise TypeError("q_values: policy must be int32, got %s" % policy.dtype)
+            if policy.shape != (n,):
+                raise ValueError("q_values: policy must have shape (%d,), got %s" % (n, policy.shape))
+            policy = np.ascontiguousarray(policy)
+            pp = policy.ctypes.data_as(C.POINTER(C.c_int32))
+        out = np.empty((n, T, A), dtype=np.float64)
+        check(self.L.rlm_eval_q(self.h, vp, pp, n, out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
 
     def set_profiling(self, on):
         check(self.L.rlm_set_profiling(self.h, 1 if on else 0))

@@ -5,6 +5,7 @@ machines without the reference can check against them).
   --reference-checks   only the fixtures of reference_checks() below
   --day-markets        only tests/golden/day_markets.json and its digests (day_market_fixtures())
   --eval-days          only tests/golden/eval_days.json and its digests (eval_days_fixtures())
+  --q-values           only tests/golden/q_values.json (tools/ref_q_values.cpp on the reference: Agent::getQ / getQb)
 
   tests/golden/units.json          reference unit-level vectors (oracle/_ref/ref_units)
   tests/golden/steps_<name>.bin    first N rlm_step_record of a reference run (oracle/_ref/ref_driver)
@@ -455,8 +456,37 @@ def eval_days_fixtures():
         json.dump(out, f, indent=1)
 
 
+def build_ref_q_values():
+    """Compile tools/ref_q_values.cpp against the reference objects oracle/Makefile built into oracle/_ref/obj, with that
+    recipe's flags (REF, as there, is where the reference sources lie) -> oracle/_ref/ref_q_values."""
+    import glob
+    ref = os.environ.get("REF", "/root/reference")
+    objs = sorted(glob.glob(os.path.join(ol.REF_DIR, "obj", "**", "*.o"), recursive=True))
+    if not objs or not os.path.exists(os.path.join(ref, "include", "rl", "agent.h")):
+        raise SystemExit("--q-values needs the reference sources ($REF) and oracle/_ref/obj (make -C oracle all)")
+    spdlog = subprocess.check_output([sys.executable, "-c", "import flashinfer, os; print(os.path.join(os.path.dirname("
+                                      "flashinfer.__file__), 'data', 'spdlog', 'include'))"]).decode().strip()
+    exe = os.path.join(ol.REF_DIR, "ref_q_values")
+    subprocess.check_call([os.environ.get("CXX", "g++"), "-std=c++11", "-O3", "-DNDEBUG", "-ffp-contract=off", "-fPIC", "-w",
+                           "-I" + os.path.join(ref, "include"), "-I" + os.path.join(ROOT, "oracle", "shim"), "-I" + spdlog,
+                           "-I" + os.path.join(ROOT, "include"), "-include", "spdlog/spdlog.h",
+                           "-include", "spdlog/sinks/rotating_file_sink.h", os.path.join(ROOT, "tools", "ref_q_values.cpp")]
+                          + objs + ["-o", exe, "-lpthread"])
+    return exe
+
+
+def q_values_fixture():
+    """getQ / getQb of the reference's QLearn / DoubleQLearn on random_init tables for a list of states."""
+    doc = subprocess.check_output([build_ref_q_values()]).decode()
+    json.loads(doc)
+    with open(os.path.join(GOLD, "q_values.json"), "w") as f:
+        f.write(doc)
+
+
 if __name__ == "__main__":
-    if sys.argv[1:] == ["--reference-checks"]:
+    if sys.argv[1:] == ["--q-values"]:
+        q_values_fixture()
+    elif sys.argv[1:] == ["--reference-checks"]:
         reference_checks()
     elif sys.argv[1:] == ["--day-markets"]:
         day_market_fixtures()
