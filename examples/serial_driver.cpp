@@ -4,6 +4,7 @@
 //
 //   g++ -std=c++17 -Iinclude examples/serial_driver.cpp -Lrl_markets_b200 -lrlm -Wl,-rpath,$PWD/rl_markets_b200 -o examples/serial_driver
 //   examples/serial_driver [--episodes N] [--algo q_learn|sarsa|double_q_learn] [--memory-size M] [--open-ticks T] [--theta out.bin]
+//                          [--flow-seed S] [--eps-T T] [--train-log-dir D]
 //                          [--md depth.csv --tas trades.csv [--symbol AAL.L] [--seed S] [--env E]]
 //                          [--test-seed S]... [--test-md depth.csv --test-tas trades.csv]...
 //
@@ -11,7 +12,9 @@
 // every episode is Intraday::LoadData(symbol, md, tas) + RunEpisode on that CSV pair (tape source), like src/main.cpp's
 // loop over its file sample; --seed sets debug.random_seed and --env the env index the seeds are derived from.
 // Prints one JSON line per episode (steps, reward, pnl) and optionally dumps theta; tests/test_gpu_facade.py and
-// tests/test_gpu_tape.py check it against the fused rlm_run_ticks path.
+// tests/test_gpu_tape.py check it against the fused rlm_run_ticks path.  --flow-seed sets the synthetic day's flow seed
+// (default 41), --eps-T policy.eps_T.  --train-log-dir D writes D/model_log.csv and D/training_log.csv as main.cpp does
+// into its output_dir with logging.log_learning on (tests/test_gpu_facade_training_logs.py).
 //
 // Test days (main.cpp:216-244): GoGreedy, ONE new Intraday, then per test day LoadData + a Backtester's RunEpisode on that
 // object.  --test-seed S (repeatable) is a synthetic day of flow seed S laid out like the training day; --test-md/--test-tas
@@ -28,7 +31,8 @@
 int main(int argc, char** argv) {
   int episodes = 2, algo = RLM_ALGO_Q_LEARN, open_ticks = 400;
   long long memory_size = 8192, seed = -1, env_index = 0;
-  std::string theta_out, md, tas, symbol = "AAL.L";
+  long long flow_seed = 41, eps_T = -1;
+  std::string theta_out, md, tas, symbol = "AAL.L", log_dir;
   std::vector<long long> test_seeds;
   std::vector<std::string> test_md, test_tas;
   for (int i = 1; i < argc; ++i) {
@@ -43,6 +47,9 @@ int main(int argc, char** argv) {
     else if (a == "--symbol") symbol = next();
     else if (a == "--seed") seed = atoll(next().c_str());
     else if (a == "--env") env_index = atoll(next().c_str());
+    else if (a == "--flow-seed") flow_seed = atoll(next().c_str());
+    else if (a == "--eps-T") eps_T = atoll(next().c_str());
+    else if (a == "--train-log-dir") log_dir = next();
     else if (a == "--test-seed") test_seeds.push_back(atoll(next().c_str()));
     else if (a == "--test-md") test_md.push_back(next());
     else if (a == "--test-tas") test_tas.push_back(next());
@@ -53,7 +60,8 @@ int main(int argc, char** argv) {
     rlm::check(rlm_config_default(&c));      // config/example.yaml
     c.algorithm = algo;
     c.memory_size = memory_size;
-    c.flow.seed = 41;
+    c.flow.seed = (uint64_t)flow_seed;
+    if (eps_T > 0) c.eps_T = (uint32_t)eps_T;
     c.flow.t0_ms = (int32_t)(c.close_ms - 30 * 60000 - (long long)open_ticks * c.flow.dt_ms);  // a short day: it closes after open_ticks rows
     if (seed >= 0) c.random_seed = (uint32_t)seed;
     c.env_index0 = env_index;
@@ -65,8 +73,8 @@ int main(int argc, char** argv) {
                                       : "a Session that trains on synthetic days tests on synthetic days (--test-seed)");
     rlm::Session session(c, csv ? RLM_SOURCE_TAPE : RLM_SOURCE_GENERATOR);
     rlm::environment::Intraday env(session);
-    rlm::rl::Agent m(session);
-    rlm::experiment::serial::Learner experiment(env);
+    rlm::rl::Agent m(session, log_dir);                      // (log_dir empty: no logs, as with log_learning off)
+    rlm::experiment::serial::Learner experiment(env, log_dir);
     for (int episode = 1; episode <= episodes; ++episode) {   // train(), main.cpp:53-78
       if (csv) env.LoadData(symbol, md, tas);
       else env.LoadData();

@@ -24,6 +24,8 @@
  *   rlm_go_greedy         Agent::GoGreedy                                  src/rl/agent.cpp:76-79
  *   rlm_read_theta        Agent::write_theta (raw double[MEMORY_SIZE])     src/rl/agent.cpp:176-181
  *   rlm_eval_q            Agent::getQ / DoubleAgent::getQb on any states   src/rl/agent.cpp:117-135,211-230
+ *   rlm_set_model_log     the model_log of Agent::HandleTransition          src/rl/agent.cpp:86-101
+ *   rlm_get_policy_descr  Policy::descr (training_log's last column)        src/rl/policy.cpp:18,77,117
  *   rlm_get_stats         Base::getEpisodeReward/getEpisodePnL/...         src/environment/base.cpp:244-252,458-473
  *
  * Conventions: plain C types only; every call returns 0 on success or a
@@ -264,6 +266,34 @@ int rlm_get_occupancy(rlm_handle h, int32_t* out /* [n_envs] */);
 
 int rlm_handle_terminal(rlm_handle h, int32_t episode);
 int rlm_go_greedy(rlm_handle h);
+
+/* ---- training logs (logging.log_learning): model_log.csv and training_log.csv ---------------------------------------
+ * model_log: Agent::HandleTransition (src/rl/agent.cpp:86-101) adds abs(delta) of every update to _agg_delta and on every
+ * 1000th update logs _agg_delta / 1000 and resets _agg_delta and _update_counter; nothing else resets them, so the count
+ * runs across episodes.  rlm_set_model_log(h, cap_rows > 0) keeps that state per env on the device, starting from the
+ * Agent constructor's (0.0, 0) with the env's next update, and a buffer of cap_rows logged values per env; after every
+ * training learner launch one small kernel folds each env's new update in, in the env's own step order, so the values are
+ * bitwise the reference's.  Turned on right after rlm_create, env b's rows are the model_log.csv of the reference process
+ * env b stands for.  cap_rows = 0 turns the log off and frees the buffers (nothing is launched while it is off).  The call
+ * waits for the handle's work; cap_rows < 0 is RLM_ERR_INVALID_ARGUMENT, RLM_ENGINE=F|f|p RLM_ERR_UNSUPPORTED.
+ * - Counted: rlm_run_ticks in train mode (tick-synchronous and round-paced engines, with or without CUDA graphs), shared-
+ *   policy training (rlm_shared_tick_accumulate + rlm_apply_dtheta, one pass after the latter) and rlm_agent_update in
+ *   train mode.  Backtest steps never count (Backtester does not call HandleTransition): entering train mode re-baselines.
+ * - The accumulators survive rlm_handle_terminal, rlm_reset, rlm_new_env and mode switches, as _update_counter does.
+ * - Shared policy: env b's rows are what its thread would log with a counter of its own.  The reference's threads share
+ *   one Agent and so one unsynchronised _agg_delta / _update_counter (a data race upstream); that interleaving is not
+ *   reproduced.
+ * - An env that completed more than one update between two passes would have lost deltas: rlm_sync reports a device
+ *   error then (no supported call sequence does this). */
+int rlm_set_model_log(rlm_handle h, int64_t cap_rows);
+/* Drain the rows of envs env0 .. env0+n-1: rows[i][0 .. n_rows[i]) (rows is [n][cap_rows]) are env env0 + i's values since
+ * the last read, in the order they were logged.  More than cap_rows values of one env between two reads: the first cap_rows
+ * are returned, every env of the range is drained all the same, and the call returns RLM_ERR_RUNTIME saying how many were
+ * lost.  RLM_ERR_INVALID_ARGUMENT (nothing written) for a null pointer, a range outside [0, n_envs) or a log that is off. */
+int rlm_read_model_log(rlm_handle h, int32_t env0, int32_t n, double* rows /* [n][cap_rows] */, int32_t* n_rows /* [n] */);
+/* Policy::descr() (src/rl/policy.cpp:18,77,117) -- the last column of training_log.csv: eps (epsilon_greedy) or tau
+ * (boltzmann) as rlm_handle_terminal last set them, 0 for the greedy and random policies and after rlm_go_greedy. */
+int rlm_get_policy_descr(rlm_handle h, double* out);
 
 /* theta access: policy = env index (independent) or 0 (shared); table 0 = A, 1 = B (double agents). */
 int rlm_read_theta(rlm_handle h, int32_t policy, int32_t table, double* out, int64_t n);

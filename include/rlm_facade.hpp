@@ -12,6 +12,9 @@
 #ifndef RLM_FACADE_HPP
 #define RLM_FACADE_HPP
 
+#include <charconv>
+#include <cmath>
+#include <cstdio>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -27,6 +30,34 @@ inline void check(int rc) {  // the reference throws std::runtime_error / std::i
   const std::string msg = rlm_last_error();
   if (rc == RLM_ERR_INVALID_ARGUMENT) throw std::invalid_argument(msg);
   throw std::runtime_error(msg);
+}
+
+// A number as the training logs print it: fmt's "{}" through spdlog's "%v" pattern, i.e. the shortest string that reads
+// back to the same double, integral values below 1e15 without a decimal point, exponents as e-05 / e+16 -- the rendering
+// of rl_markets_b200/backtest.py's _num, which the reference's files are checked against.
+inline std::string log_num(double x) {
+  if (std::isnan(x)) return "nan";
+  if (std::isinf(x)) return x < 0 ? "-inf" : "inf";
+  if (x == std::trunc(x) && std::fabs(x) < 1e15) return std::to_string((long long)x);
+  char buf[64];
+  const auto r = std::to_chars(buf, buf + sizeof(buf), x, std::chars_format::scientific);  // shortest d.ddde+XX
+  const std::string sci(buf, r.ptr);
+  const size_t e = sci.find('e');
+  const int ex = std::stoi(sci.substr(e + 1));
+  const bool neg = sci[0] == '-';
+  std::string digits;
+  for (size_t i = neg ? 1 : 0; i < e; ++i) if (sci[i] != '.') digits += sci[i];
+  std::string out = neg ? "-" : "";
+  if (ex < -4 || ex >= 16) {  // repr's scientific form
+    out += digits.substr(0, 1);
+    if (digits.size() > 1) out += "." + digits.substr(1);
+    char eb[16];
+    snprintf(eb, sizeof(eb), "e%c%02d", ex < 0 ? '-' : '+', ex < 0 ? -ex : ex);
+    return out + eb;
+  }
+  if (ex < 0) return out + "0." + std::string((size_t)(-ex - 1), '0') + digits;
+  if ((size_t)ex + 1 >= digits.size()) return out + digits + std::string((size_t)ex + 1 - digits.size(), '0') + ".0";
+  return out + digits.substr(0, (size_t)ex + 1) + "." + digits.substr((size_t)ex + 1);
 }
 
 // one env + one agent + the Runner's States: a library handle with n_envs = 1.  source: RLM_SOURCE_GENERATOR (the synthetic
@@ -69,6 +100,7 @@ class Intraday {
   void LoadData(const rlm_flow_params* day = nullptr) {
     if (!day) return;
     check(rlm_set_flow(s_.handle(), day));
+    date_ = day->date;
     started_ = true;  // (the next Initialise resets the envs onto the new day's flow)
   }
   // Intraday::LoadData(ticker, md_path, tas_path) (intraday.cpp:141-150) on a tape Session: the CSV pair is read by
@@ -83,8 +115,11 @@ class Intraday {
     const int64_t offsets[2] = {0, n};
     check(rlm_load_days(s_.handle(), msgs.data(), offsets, 1));
     ticker_ = ticker;
+    date_ = n > 0 ? msgs[0].date : 0;
   }
   const std::string& ticker() const { return ticker_; }
+  // Intraday::getEpisodeId (intraday.cpp:160): to_string(init_date), the date of the day the episode runs on
+  std::string getEpisodeId() const { return std::to_string(date_); }
   // Intraday::Initialise (intraday.cpp:103-138): rows until the open, then until every window is full
   bool Initialise() {
     if (started_) check(rlm_reset(s_.handle()));
@@ -123,6 +158,7 @@ class Intraday {
   double reward_ = 0.0;
   bool terminal_ = false, started_ = false;
   std::string ticker_;
+  int date_ = s_.config().flow.date;  // (a generator Session's day; LoadData replaces it)
 };
 
 }  // namespace environment
@@ -133,6 +169,33 @@ namespace rl {
 class Agent {
  public:
   explicit Agent(Session& s) : s_(s) {}
+  // Agent::Agent with logging.log_learning on (agent.cpp:52-59): `output_dir` + "model_log.csv" receives _agg_delta / 1000
+  // on every 1000th update (agent.cpp:86-101).  The values are accumulated on the device (rlm_set_model_log) and written
+  // out by FlushModelLog, which Learner::RunEpisode calls after every episode.  Build the Agent on a fresh Session for a
+  // file equal to the reference's.
+  Agent(Session& s, const std::string& output_dir) : s_(s) {
+    if (output_dir.empty()) return;
+    check(rlm_set_model_log(s_.handle(), kModelLogCap));
+    model_log_ = output_dir + "/model_log.csv";
+    FILE* f = fopen(model_log_.c_str(), "w");
+    if (!f) throw std::runtime_error("cannot open " + model_log_);
+    fclose(f);
+  }
+  void FlushModelLog() {
+    if (model_log_.empty()) return;
+    std::vector<double> rows(kModelLogCap);
+    int32_t n = 0;
+    check(rlm_read_model_log(s_.handle(), 0, 1, rows.data(), &n));
+    FILE* f = fopen(model_log_.c_str(), "a");
+    if (!f) throw std::runtime_error("cannot open " + model_log_);
+    for (int32_t i = 0; i < n; ++i) fprintf(f, "%s\n", log_num(rows[i]).c_str());
+    fclose(f);
+  }
+  double descr() const {                                   // Policy::descr() of the agent's policy (policy.cpp:18,77,117)
+    double d = 0.0;
+    check(rlm_get_policy_descr(s_.handle(), &d));
+    return d;
+  }
   int action() {                                           // Agent::action(State&) (agent.cpp:60-74)
     int32_t a = -1;
     check(rlm_act(s_.handle(), &a));
@@ -165,7 +228,9 @@ class Agent {
     check(rlm_eval_q(s_.handle(), vars.data(), nullptr, 1, out));
     return out[table * c.n_actions + action];
   }
+  static constexpr int64_t kModelLogCap = 1 << 16;  // values kept between two flushes (one per 1000 updates)
   Session& s_;
+  std::string model_log_;
 };
 
 }  // namespace rl
@@ -177,6 +242,16 @@ namespace serial {
 class Learner {
  public:
   Learner(environment::Intraday& env) : environment(env) {}
+  // Learner::Learner with logging.log_learning on (serial.cpp:40-50): `output_dir` + "training_log.csv" gets the header,
+  // then one row per episode (:81-88).  Pair it with rl::Agent(session, output_dir) for the model_log.
+  Learner(environment::Intraday& env, const std::string& output_dir) : environment(env) {
+    if (output_dir.empty()) return;
+    training_log_ = output_dir + "/training_log.csv";
+    FILE* f = fopen(training_log_.c_str(), "w");
+    if (!f) throw std::runtime_error("cannot open " + training_log_);
+    fprintf(f, "episode,episode_id,reward,pnl,n_steps,epsilon\n");
+    fclose(f);
+  }
   bool RunEpisode(rl::Agent* m) {
     _step_counter = 0;
     if (!environment.Initialise()) return false;           // Runner::RunEpisode, serial.cpp:20-22
@@ -184,6 +259,14 @@ class Learner {
     do { is_terminal = _step(m); } while (!is_terminal);   // :27-29
     environment.ClearInventory();                          // :31
     m->HandleTerminal(_episode_counter++);                 // Learner::RunEpisode, :79
+    if (!training_log_.empty()) {                          // :81-88
+      FILE* f = fopen(training_log_.c_str(), "a");
+      if (!f) throw std::runtime_error("cannot open " + training_log_);
+      fprintf(f, "%d,%s,%s,%s,%ld,%s\n", _episode_counter, environment.getEpisodeId().c_str(), log_num(environment.getEpisodeReward()).c_str(),
+              log_num(environment.getEpisodePnL()).c_str(), _step_counter, log_num(m->descr()).c_str());
+      fclose(f);
+    }
+    m->FlushModelLog();
     return true;
   }
   long steps() const { return _step_counter; }
@@ -200,6 +283,7 @@ class Learner {
   environment::Intraday& environment;
   long _step_counter = 0;
   int _episode_counter = 0;
+  std::string training_log_;
 };
 
 // experiment::serial::Backtester (src/experiment/serial.cpp:97-137): the greedy evaluation of main.cpp:216-244.  The

@@ -97,6 +97,9 @@ struct rlm_handle_s {
   int* h_live = nullptr;  // pinned [RLM_MAX_SUB][2]: ready count of the last round of each group in flight
   cudaEvent_t ev_live[RLM_MAX_SUB][2] = {};
   long long rounds_launched = 0, rounds_calls = 0;
+  // model_log (rlm_set_model_log): off while mlog.cap == 0; then one rlm_model_log_kernel pass follows every training
+  // learner launch
+  ModelLogPtrs mlog = {};
 };
 
 // The kernels read their per-handle constants from ONE __constant__ block (rlm_env.cuh: P).  g_params_owner says whose
@@ -302,6 +305,14 @@ static cudaError_t launch_agent_on(rlm_handle_s* h, const DevPtrs& ptr, const Dy
 }
 static cudaError_t launch_agent_any(rlm_handle_s* h, const DynParams& d, int tslot, int stage) {
   return launch_agent_on(h, h->ptr, d, tslot, stage, h->stream);
+}
+// model_log: the accumulation pass over envs env0 .. env0+n-1 after a learner launch of training (HandleTransition's
+// _agg_delta / _update_counter).  Nothing is launched while the log is off or in backtest mode (Backtester::_step never
+// calls HandleTransition); *launched counts what was.
+static cudaError_t model_log_pass(rlm_handle_s* h, const DynParams& d, int env0, int n, cudaStream_t st, long long* launched) {
+  if (h->mlog.cap == 0 || d.backtest) return cudaSuccess;
+  ++*launched;
+  return rlm_launch_model_log(h->mlog, h->ptr, h->hp.env_stride, env0, n, st);
 }
 
 static int upload_params(rlm_handle_s* h) {
@@ -530,6 +541,7 @@ int rlm_destroy(rlm_handle h) {
   cudaFree((void*)h->dm.markets); cudaFree(h->dm.env_market); cudaFree(h->dm.rec_fixed);
   for (auto& es : h->ev_live) for (auto e : es) if (e) cudaEventDestroy(e);
   cudaFree(h->ptr.q_slots); cudaFree(h->ptr.ag_done); cudaFree(h->d_qctl);
+  cudaFree(h->mlog.acc); cudaFree(h->mlog.written); cudaFree(h->mlog.rows);
   for (auto e : h->ev) cudaEventDestroy(e);
   for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
@@ -570,6 +582,12 @@ int rlm_set_mode(rlm_handle h, int32_t mode) {
   if (mode != RLM_MODE_TRAIN && mode != RLM_MODE_BACKTEST) return fail(RLM_ERR_INVALID_ARGUMENT, "unknown mode");
   if (mode == RLM_MODE_BACKTEST && h->engine != 1 && h->engine != 3) return fail(RLM_ERR_UNSUPPORTED, "backtest mode runs on the tick-synchronous engine only");
   if (h->dyn.backtest != mode) h->graph_warm = false;  // (the other mode's kernel: its first call launches directly, see run_ticks_impl)
+  if (h->mlog.cap > 0 && h->dyn.backtest && mode == RLM_MODE_TRAIN) {
+    // back to training: the evaluation steps moved n_steps without a HandleTransition
+    API_LOCK;
+    CK(cudaSetDevice(h->cfg.device));
+    CK(rlm_launch_model_log_baseline(h->mlog, h->ptr, h->hp.env_stride, h->cfg.n_envs, h->stream));
+  }
   h->dyn.backtest = mode;
   return RLM_OK;
 }
@@ -886,6 +904,7 @@ static int run_rounds_impl(rlm_handle h, const DynParams& d, int n_ticks) {
   DynParams dts[RLM_MAX_SUB];
   DevPtrs pss[RLM_MAX_SUB];
   cudaGraphExec_t exec[RLM_MAX_SUB] = {};
+  long long ml_captured = 0;  // (a graph's model_log passes are counted when it is launched)
   if (S > 1) CK(cudaEventRecord(h->ev_fork, h->stream));
   for (int s = 0; s < S; ++s) {
     cudaStream_t st = S > 1 ? h->sub_stream[s] : h->stream;
@@ -915,6 +934,7 @@ static int run_rounds_impl(rlm_handle h, const DynParams& d, int n_ticks) {
       for (int r = 0; r < G && ce == cudaSuccess; ++r) {
         ce = rlm_launch_env_round(ps, dt, dt.n_sub, r, st);
         if (ce == cudaSuccess) ce = launch_agent_on(h, ps, dt, r, 0, st);
+        if (ce == cudaSuccess) ce = model_log_pass(h, dt, dt.env0, dt.n_sub, st, &ml_captured);
       }
       cudaError_t ce2 = cudaStreamEndCapture(st, &graph);
       if (ce != cudaSuccess || ce2 != cudaSuccess) { if (graph) cudaGraphDestroy(graph); CK(ce != cudaSuccess ? ce : ce2); }
@@ -943,6 +963,7 @@ static int run_rounds_impl(rlm_handle h, const DynParams& d, int n_ticks) {
           if (h->profile) CK(cudaEventRecord(h->ev[3 * r + 1], st));
           CK(launch_agent_on(h, pss[s], dts[s], r, 0, st));
           if (h->profile) CK(cudaEventRecord(h->ev[3 * r + 2], st));
+          CK(model_log_pass(h, dts[s], dts[s].env0, dts[s].n_sub, st, &h->launches));
         }
         if (h->profile) {  // bench instrumentation: per-kernel times of the rounds that had work (S == 1, direct launches)
           std::vector<int> cnt(2 * G);
@@ -959,6 +980,7 @@ static int run_rounds_impl(rlm_handle h, const DynParams& d, int n_ticks) {
         }
       }
       h->launches += 2 * G;
+      if (exec[s]) h->launches += h->mlog.cap > 0 ? G : 0;  // (the graph's model_log passes)
       h->rounds_launched += G;
       CK(cudaMemcpyAsync(h->h_live + 2 * s + (k & 1), pss[s].ready_count + RLM_LIVE_OFF + (G - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
       CK(cudaEventRecord(h->ev_live[s][k & 1], st));
@@ -1063,6 +1085,7 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
       CK(rlm_launch_runctl(h->ptr, rc, h->stream));
     }
     rlm_handle_s::TickGraph* tg = nullptr;
+    long long ml_dummy = 0;
     for (auto& g : h->graphs)
       if (g.chunk == chunk && memcmp(&g.d, &dt, sizeof(DynParams)) == 0) tg = &g;
     if (!tg) {
@@ -1073,6 +1096,7 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
       for (int t = 0; t < chunk && ce == cudaSuccess; ++t) {
         ce = rlm_launch_env(pg, dt, B, t, 0, h->env_variant, h->stream);
         if (ce == cudaSuccess) ce = launch_agent_on(h, pg, dt, t, 0, h->stream);
+        if (ce == cudaSuccess) ce = model_log_pass(h, dt, 0, B, h->stream, &ml_dummy);
       }
       cudaError_t ce2 = cudaStreamEndCapture(h->stream, &graph);
       if (ce != cudaSuccess || ce2 != cudaSuccess) { if (graph) cudaGraphDestroy(graph); CK(ce != cudaSuccess ? ce : ce2); }
@@ -1085,6 +1109,7 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
     }
     CK(cudaGraphLaunch(tg->exec, h->stream));
     h->launches += 2 * chunk;
+    if (h->mlog.cap > 0 && !d.backtest) h->launches += chunk;  // (the graph's model_log passes)
     done += chunk;
   }
   while (done < n_ticks) {
@@ -1112,6 +1137,7 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
         CK(launch_agent_on(h, ps, dt, t, 0, st));
         if (h->profile) CK(cudaEventRecord(h->ev[3 * t + 2], st));
         h->launches += 2;
+        CK(model_log_pass(h, dt, dt.env0, dt.n_sub, st, &h->launches));
       }
     }
     if (h->profile) {
@@ -1151,13 +1177,14 @@ int rlm_sync(rlm_handle h) {
   CK(cudaMemcpy(c, h->ptr.counters, sizeof(c), cudaMemcpyDeviceToHost));
   unsigned err = (unsigned)c[4];
   if (err) {
-    char buf[256];
-    snprintf(buf, sizeof(buf), "device error flags 0x%x:%s%s%s%s%s", err,
+    char buf[512];
+    snprintf(buf, sizeof(buf), "device error flags 0x%x:%s%s%s%s%s%s", err,
              (err & ERR_BAD_PRICE) ? " non-positive price/volume (book.cpp:74-77)" : "",
              (err & ERR_TICK_RANGE) ? " invalid price/ticks for conversion (market.cpp:86,112)" : "",
              (err & ERR_TRACE_OVERFLOW) ? " trace list overflow (raise trace_cap)" : "",
              (err & ERR_INVALID_STATE) ? " invalid book state (book.cpp:612-625)" : "",
-             (err & ERR_STREAM_UNDERRUN) ? " stream underrun" : "");
+             (err & ERR_STREAM_UNDERRUN) ? " stream underrun" : "",
+             (err & ERR_MODEL_LOG_GAP) ? " model_log: an env completed more than one update between two accumulation passes (deltas lost)" : "");
     return fail((err & ERR_TICK_RANGE) ? RLM_ERR_INVALID_ARGUMENT : RLM_ERR_RUNTIME, buf);
   }
   return RLM_OK;
@@ -1273,6 +1300,82 @@ int rlm_handle_terminal(rlm_handle h, int32_t episode) {
     double t0 = (double)c.tau_init, tf = (double)c.tau_floor;
     h->tau = t0 * pow(tf / t0, (double)episode / (double)(long)c.tau_T);
   }
+  return RLM_OK;
+}
+
+// ---- model_log / training_log (Agent::HandleTransition, agent.cpp:86-101; Learner::RunEpisode, serial.cpp:72-94) ----
+int rlm_set_model_log(rlm_handle h, int64_t cap_rows) {
+  API_LOCK;
+  if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
+  if (cap_rows < 0) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_set_model_log: cap_rows < 0");
+  if (cap_rows > 0 && h->engine != 1)
+    return fail(RLM_ERR_UNSUPPORTED, "rlm_set_model_log: RLM_ENGINE=F|f|p run every step inside one launch; the model_log needs the "
+                                     "tick-synchronous or round-paced engine");
+  const double need = (double)h->cfg.n_envs * ((double)cap_rows * 8.0 + sizeof(ModelLogAcc) + 8.0);
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  if (cap_rows > 0) {
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    const double have = (double)free_b + (double)h->cfg.n_envs * ((double)h->mlog.cap * 8.0 + (h->mlog.cap ? sizeof(ModelLogAcc) + 8.0 : 0.0));
+    if (need > have)
+      return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_set_model_log: n_envs x cap_rows needs " + std::to_string((long long)(need / 1e6)) +
+                                                " MB of device memory, " + std::to_string((long long)(have / 1e6)) + " MB are free");
+  }
+  // the cached CUDA graphs were captured with (or without) the accumulation pass and its buffers
+  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
+  h->graphs.clear();
+  cudaFree(h->mlog.acc); cudaFree(h->mlog.written); cudaFree(h->mlog.rows);
+  h->mlog = ModelLogPtrs{};
+  if (cap_rows == 0) return RLM_OK;
+  const int B = h->cfg.n_envs;
+  ModelLogPtrs L = {};
+  L.cap = cap_rows;
+  cudaError_t ce = cudaMalloc(&L.acc, (size_t)B * sizeof(ModelLogAcc));
+  if (ce == cudaSuccess) ce = cudaMalloc(&L.written, (size_t)B * 8);
+  if (ce == cudaSuccess) ce = cudaMalloc(&L.rows, (size_t)B * (size_t)cap_rows * 8);
+  // the Agent constructor's state: _agg_delta = 0.0, _update_counter = 0 (agent.h:40-41), counting from the env's next step
+  if (ce == cudaSuccess) ce = cudaMemsetAsync(L.acc, 0, (size_t)B * sizeof(ModelLogAcc), h->stream);
+  if (ce == cudaSuccess) ce = cudaMemsetAsync(L.written, 0, (size_t)B * 8, h->stream);
+  if (ce == cudaSuccess) ce = rlm_launch_model_log_baseline(L, h->ptr, h->hp.env_stride, B, h->stream);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(h->stream);
+  if (ce != cudaSuccess) { cudaFree(L.acc); cudaFree(L.written); cudaFree(L.rows); CK(ce); }
+  h->mlog = L;
+  return RLM_OK;
+}
+
+int rlm_read_model_log(rlm_handle h, int32_t env0, int32_t n, double* rows, int32_t* n_rows) {
+  API_LOCK;
+  if (!h || (n > 0 && (!rows || !n_rows))) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_read_model_log: null argument");
+  if (h->mlog.cap == 0) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_read_model_log: the model_log is off (rlm_set_model_log)");
+  if (env0 < 0 || n < 0 || (int64_t)env0 + n > h->cfg.n_envs) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_read_model_log: env range out of bounds");
+  if (n == 0) return RLM_OK;
+  CK(cudaSetDevice(h->cfg.device));
+  CK(cudaStreamSynchronize(h->stream));
+  const long long cap = h->mlog.cap;
+  std::vector<long long> w(n);
+  CK(cudaMemcpy(w.data(), h->mlog.written + env0, (size_t)n * 8, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(rows, h->mlog.rows + (size_t)env0 * cap, (size_t)n * (size_t)cap * 8, cudaMemcpyDeviceToHost));
+  // (on the handle's stream, before any later accumulation pass; the sync keeps a pass from logging into the old count)
+  CK(cudaMemsetAsync(h->mlog.written + env0, 0, (size_t)n * 8, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  long long lost = 0;
+  int first = -1;
+  for (int i = 0; i < n; ++i) {
+    n_rows[i] = (int32_t)std::min(w[i], cap);
+    if (w[i] > cap) { lost += w[i] - cap; if (first < 0) first = env0 + i; }
+  }
+  if (lost > 0)
+    return fail(RLM_ERR_RUNTIME, "rlm_read_model_log: " + std::to_string(lost) + " rows were lost (env " + std::to_string(first) +
+                                     " first): more than cap_rows = " + std::to_string(cap) + " rows were logged before this read");
+  return RLM_OK;
+}
+
+int rlm_get_policy_descr(rlm_handle h, double* out) {
+  if (!h || !out) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_get_policy_descr: null argument");
+  // Policy::descr() (policy.cpp:18,77,117); Agent::GoGreedy installs a Greedy policy, whose descr() is 0
+  const int t = h->dyn.greedy ? RLM_POLICY_GREEDY : h->cfg.policy_type;
+  *out = t == RLM_POLICY_EPSILON_GREEDY ? h->eps : (t == RLM_POLICY_BOLTZMANN ? h->tau : 0.0);
   return RLM_OK;
 }
 
@@ -1454,6 +1557,7 @@ int rlm_apply_dtheta(rlm_handle h) {
   CK(launch_agent_any(h, h->shared_dyn, 0, 2));
   CK(rlm_launch_env(h->ptr, h->shared_dyn, h->cfg.n_envs, 0, 1, h->env_variant, h->stream));
   h->launches += 3;
+  CK(model_log_pass(h, h->shared_dyn, 0, h->cfg.n_envs, h->stream, &h->launches));
   return RLM_OK;
 }
 
@@ -1553,6 +1657,7 @@ int rlm_agent_update(rlm_handle h, double* delta_out) {
   CK(launch_agent_any(h, split_dyn(h), 0, 0));
   CK(cudaMemsetAsync(h->ptr.ready_count, 0, 4, h->stream));
   h->launches += 1;
+  CK(model_log_pass(h, h->dyn, 0, B, h->stream, &h->launches));
   if (delta_out && h->dyn.backtest) {
     // Backtester::_step computes no TD error (AgentD::last_delta may still hold the last one of training)
     memset(delta_out, 0, (size_t)B * 8);

@@ -35,6 +35,8 @@ cudaError_t rlm_launch_gather(const DevPtrs& ptr, int n_envs, int what, void* ou
 cudaError_t rlm_launch_clear_traces(const DevPtrs& ptr, int n_envs, cudaStream_t st);
 cudaError_t rlm_launch_env_market(const DevPtrs& ptr, int env0, int n, const int* mk, cudaStream_t st);
 cudaError_t rlm_launch_fix_terminal(const DevPtrs& ptr, int record_envs, cudaStream_t st);
+cudaError_t rlm_launch_model_log(const ModelLogPtrs& L, const DevPtrs& ptr, int env_stride, int env0, int n, cudaStream_t st);
+cudaError_t rlm_launch_model_log_baseline(const ModelLogPtrs& L, const DevPtrs& ptr, int env_stride, int n_envs, cudaStream_t st);
 cudaError_t rlm_launch_test_to_ticks(const double* px, int n, int* out);
 cudaError_t rlm_launch_test_to_price(const int* t, int n, double* out);
 cudaError_t rlm_launch_test_tiles(const float* vars, int n, int* out);

@@ -21,7 +21,8 @@ enum {
   ERR_TICK_RANGE = 2,      // market.cpp:86,112 invalid price / tick for conversion
   ERR_TRACE_OVERFLOW = 4,  // more nonzero traces than trace_cap (traces.h:13 MAX_NONZERO_TRACES analogue)
   ERR_INVALID_STATE = 8,   // BookUtils::IsValidState false (the reference would merge rows)
-  ERR_STREAM_UNDERRUN = 16
+  ERR_STREAM_UNDERRUN = 16,
+  ERR_MODEL_LOG_GAP = 32   // model_log: an env completed more than one update between two accumulation passes
 };
 
 struct OrderD {  // market::Order (include/market/order.h:11-51); one per side (ORDER_LIMIT == 1, base.cpp:21)
@@ -198,6 +199,21 @@ struct DevPtrs {
   const rlm_tick_msg* tape;      // [n_msgs] concatenated days
   int2* tape_cur;                // [n_envs] {next message, end of the env's day} (absolute message indices)
   int* tape_lo;                  // [n_envs] first message of the env's day (rlm_reset / rlm_new_env rewind to it)
+};
+
+// model_log (rlm_set_model_log, rlm_model_log.cu): per env the state of Agent::_agg_delta / _update_counter
+// (include/rl/agent.h:40-41) and the rows it has logged since the last read
+struct ModelLogAcc {
+  double agg;      // _agg_delta
+  long long seen;  // AgentD::n_steps at the last pass
+  int count;       // _update_counter
+  int pad;
+};
+struct ModelLogPtrs {
+  ModelLogAcc* acc;    // [n_envs]
+  long long* written;  // [n_envs] rows logged since the last read (the first `cap` of them are kept)
+  double* rows;        // [n_envs][cap]
+  long long cap;
 };
 
 // Tape days with markets of their own (rlm_set_day_markets).  A __constant__ block of its own (rlm_env.cuh: PM), uploaded

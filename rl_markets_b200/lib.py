@@ -16,7 +16,7 @@ EXPORTS = [
     "rlm_last_error", "rlm_abi_version", "rlm_config_default", "rlm_create", "rlm_destroy", "rlm_reset", "rlm_set_mode", "rlm_new_env", "rlm_set_flow",
     "rlm_load_ticks", "rlm_load_days", "rlm_assign_days", "rlm_get_tape_pos", "rlm_set_day_markets", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
     "rlm_get_reward", "rlm_get_actions", "rlm_get_rho", "rlm_get_occupancy", "rlm_copy_theta", "rlm_handle_terminal", "rlm_go_greedy", "rlm_read_theta",
-    "rlm_write_theta", "rlm_eval_q", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
+    "rlm_write_theta", "rlm_eval_q", "rlm_set_model_log", "rlm_read_model_log", "rlm_get_policy_descr", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
     "rlm_set_stream", "rlm_set_profiling", "rlm_get_kernel_times", "rlm_act", "rlm_env_step", "rlm_agent_update", "rlm_ingest_csv",
     "rlm_flow_generate", "rlm_test_to_ticks", "rlm_test_to_price", "rlm_test_tiles", "rlm_test_learner_tiles", "rlm_test_order",
     "rlm_test_rolling_mean",
@@ -71,6 +71,9 @@ def load():
     L.rlm_read_theta.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), C.c_int64]
     L.rlm_write_theta.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), C.c_int64]
     L.rlm_eval_q.argtypes = [C.c_void_p, P(C.c_float), P(C.c_int32), C.c_int64, P(C.c_double)]
+    L.rlm_set_model_log.argtypes = [C.c_void_p, C.c_int64]
+    L.rlm_read_model_log.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), P(C.c_int32)]
+    L.rlm_get_policy_descr.argtypes = [C.c_void_p, P(C.c_double)]
     L.rlm_read_records.argtypes = [C.c_void_p, C.c_int32, P(abi.StepRecord), C.c_int32, P(C.c_int32)]
     L.rlm_device_ptrs.argtypes = [C.c_void_p, P(C.c_void_p), P(C.c_void_p), P(C.c_int64)]
     L.rlm_apply_dtheta.argtypes = [C.c_void_p]
@@ -313,6 +316,32 @@ class BatchedMarket:
         out = np.empty((n, T, A), dtype=np.float64)
         check(self.L.rlm_eval_q(self.h, vp, pp, n, out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
+
+    # ---- training logs (logging.log_learning; rl_markets_b200/train_logs.py writes the files)
+    def set_model_log(self, cap_rows):
+        """Agent::HandleTransition's model_log on the device: cap_rows > 0 keeps up to cap_rows logged values per env between
+        two model_log() reads, starting from the Agent constructor's state; 0 turns it off (rlm_set_model_log)."""
+        if not isinstance(cap_rows, int) or isinstance(cap_rows, bool):
+            raise TypeError("set_model_log: cap_rows must be an int, got %r" % (cap_rows,))
+        check(self.L.rlm_set_model_log(self.h, cap_rows))
+        self._mlog_cap = cap_rows
+
+    def model_log(self, env0=0, n=None):
+        """Drain the model_log of envs env0 .. env0+n-1: one list of floats per env (_agg_delta / 1000 of every 1000th
+        update since the last read, in order).  Raises RlmError when an env logged more than cap_rows values in between."""
+        n = self.cfg.n_envs - env0 if n is None else n
+        cap = getattr(self, "_mlog_cap", 0)
+        rows = (C.c_double * max(n * cap, 1))()
+        cnt = (C.c_int32 * max(n, 1))()
+        check(self.L.rlm_read_model_log(self.h, env0, n, rows, cnt))
+        return [[rows[i * cap + k] for k in range(cnt[i])] for i in range(n)]
+
+    def policy_descr(self):
+        """Policy::descr(): eps / tau after the last handle_terminal, 0 for greedy and random policies (training_log's last
+        column)."""
+        out = C.c_double()
+        check(self.L.rlm_get_policy_descr(self.h, C.byref(out)))
+        return out.value
 
     def set_profiling(self, on):
         check(self.L.rlm_set_profiling(self.h, 1 if on else 0))

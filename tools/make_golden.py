@@ -6,6 +6,8 @@ machines without the reference can check against them).
   --day-markets        only tests/golden/day_markets.json and its digests (day_market_fixtures())
   --eval-days          only tests/golden/eval_days.json and its digests (eval_days_fixtures())
   --q-values           only tests/golden/q_values.json (tools/ref_q_values.cpp on the reference: Agent::getQ / getQb)
+  --training-logs      only tests/golden/training_logs.json and tl_<case>_{model,training}_log.csv (tools/ref_train_logs.cpp:
+                       the reference trained with logging.log_learning on)
 
   tests/golden/units.json          reference unit-level vectors (oracle/_ref/ref_units)
   tests/golden/steps_<name>.bin    first N rlm_step_record of a reference run (oracle/_ref/ref_driver)
@@ -483,9 +485,109 @@ def q_values_fixture():
         f.write(doc)
 
 
+# Training logs (logging.log_learning): model_log.csv of Agent::HandleTransition and training_log.csv of
+# Learner::RunEpisode, written by the reference itself (tools/ref_train_logs.cpp).  A case trains one agent for `episodes`
+# episodes on one Intraday, episode e on day e % len(days) (main.cpp:45-60); a day is a synthetic stream (flow_seed,
+# ticks, open_ticks; env = the case's) or a venue day (a VENUE_CASES name, under its ticker's market).  Enough episodes
+# that several 1000-update windows close, inside episodes and spanning episode boundaries.  Written to
+# tests/golden/training_logs.json and tl_<case>_{model_log,training_log}.csv, not into manifest.json.
+def _tl(name, algo, M, env, flow_seed, over, episodes=8, days=None):
+    days = days or [dict(flow_seed=flow_seed, ticks=2100, open_ticks=1800)]
+    return dict(name=name, algo=algo, M=M, env=env, over=over, episodes=episodes, days=days)
+
+
+TRAINING_LOG_CASES = [
+    _tl("tl_q_learn_eps", "q_learn", 8192, 80, 301, {"policy.eps_T": 5}),
+    _tl("tl_sarsa_boltzmann", "sarsa", 8192, 81, 303,
+        {"policy.type": "boltzmann", "policy.tau_init": 0.05, "policy.tau_floor": 0.01, "policy.tau_T": 10}),
+    _tl("tl_double_q_greedy", "double_q_learn", 8192, 82, 305, {"policy.type": "greedy", "learning.alpha_start": 0.01}),
+    _tl("tl_r_learn", "r_learn", 8192, 83, 307, {"policy.eps_init": 0.3}),
+    _tl("tl_online_r_learn", "online_r_learn", 8192, 84, 309, {"policy.eps_init": 0.3}),
+    _tl("tl_double_r_learn", "double_r_learn", 8209, 85, 311, {"policy.eps_init": 0.3, "learning.alpha_start": 0.01}),
+    _tl("tl_q_learn_two_days", "q_learn", 5003, 86, 313, {}, episodes=9,
+        days=[dict(flow_seed=313, ticks=1500, open_ticks=1200), dict(flow_seed=314, ticks=2400, open_ticks=2100)]),
+    _tl("tl_venue_aal", "q_learn", 8192, 87, 0, {}, episodes=4, days=[dict(venue="venue_aal_l")]),
+]
+
+
+def training_logs_yaml(c, out_dir=None):
+    y = config.example_dict(**{"learning.memory_size": c["M"], "learning.algorithm": c["algo"], **c["over"]})
+    if out_dir is not None:  # Agent's / Learner's ctors open <output_dir>model_log.csv / training_log.csv
+        y["logging"] = {"log_learning": True, "max_size": 1 << 40}
+        y["output_dir"] = out_dir
+    return y
+
+
+def build_ref_train_logs():
+    """Compile tools/ref_train_logs.cpp against the reference objects oracle/Makefile built into oracle/_ref/obj, with that
+    recipe's flags -> oracle/_ref/ref_train_logs."""
+    import glob
+    ref = os.environ.get("REF", "/root/reference")
+    objs = sorted(glob.glob(os.path.join(ol.REF_DIR, "obj", "**", "*.o"), recursive=True))
+    if not objs or not os.path.exists(os.path.join(ref, "include", "rl", "agent.h")):
+        raise SystemExit("--training-logs needs the reference sources ($REF) and oracle/_ref/obj (make -C oracle all)")
+    spdlog = subprocess.check_output([sys.executable, "-c", "import flashinfer, os; print(os.path.join(os.path.dirname("
+                                      "flashinfer.__file__), 'data', 'spdlog', 'include'))"]).decode().strip()
+    exe = os.path.join(ol.REF_DIR, "ref_train_logs")
+    subprocess.check_call([os.environ.get("CXX", "g++"), "-std=c++14", "-O3", "-DNDEBUG", "-ffp-contract=off", "-fPIC", "-w",
+                           "-I" + os.path.join(ref, "include"), "-I" + os.path.join(ROOT, "oracle", "shim"), "-I" + spdlog,
+                           "-include", "spdlog/spdlog.h", "-include", "spdlog/sinks/rotating_file_sink.h",
+                           os.path.join(ROOT, "tools", "ref_train_logs.cpp")]
+                          + objs + ["-o", exe, "-lpthread"])
+    return exe
+
+
+def training_logs_fixtures():
+    import tempfile
+    import golden_util
+    exe = build_ref_train_logs()
+    venues = {v["name"]: v for v in VENUE_CASES}
+    out = []
+    for c in TRAINING_LOG_CASES:
+        y = training_logs_yaml(c)
+        cfg = config.from_dict(y)
+        with tempfile.TemporaryDirectory() as d:
+            logs = os.path.join(d, "logs") + "/"
+            os.makedirs(logs)
+            y_run = json.loads(json.dumps(training_logs_yaml(c, logs)))
+            y_run["debug"]["random_seed"] = y["debug"]["random_seed"] + c["env"]
+            cfgp = os.path.join(d, "cfg.yaml")
+            ol.write_ref_yaml(cfgp, y_run)
+            cmd, days = [exe, "--config", cfgp, "--episodes", str(c["episodes"])], []
+            for k, day in enumerate(c["days"]):
+                if "venue" in day:
+                    v = venues[day["venue"]]
+                    sub = os.path.join(d, "day%d" % k)
+                    os.makedirs(sub)
+                    md, tas = golden_util.venue_day(v, sub)
+                    days.append(dict(day, ticker=v["ticker"], md_sha256=file_sha256(md), tas_sha256=file_sha256(tas)))
+                    cmd += ["--symbol", v["ticker"], "--md", md, "--tas", tas]
+                else:
+                    t0 = day_t0(cfg, day["open_ticks"])
+                    md, tas = os.path.join(d, "d%d_md_1.csv" % k), os.path.join(d, "d%d_tas_1.csv" % k)
+                    subprocess.check_call([ol.FLOW_CSV, "--seed", str(day["flow_seed"]), "--env", str(c["env"]), "--ticks", str(day["ticks"]),
+                                           "--dt-ms", "250", "--md", md, "--tas", tas, "--t0-ms", str(t0)])
+                    days.append(dict(day, t0_ms=t0))
+                    cmd += ["--symbol", y["data"]["symbols"][0], "--md", md, "--tas", tas]
+            summary = json.loads(subprocess.check_output(cmd).decode().strip().splitlines()[-1])
+            files = {}
+            for n in ("model_log", "training_log"):
+                with open(os.path.join(logs, n + ".csv")) as f:
+                    files[n] = f.read()
+                with open(os.path.join(GOLD, "%s_%s.csv" % (c["name"], n)), "w") as f:
+                    f.write(files[n])
+        n_rows = len(files["model_log"].splitlines())
+        assert n_rows >= 2, (c["name"], n_rows)
+        out.append(dict(c, yaml=y, days=days, episode_ids=[e["episode_id"] for e in summary["episodes"]], model_log_rows=n_rows))
+    with open(os.path.join(GOLD, "training_logs.json"), "w") as f:
+        json.dump(out, f, indent=1)
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["--q-values"]:
         q_values_fixture()
+    elif sys.argv[1:] == ["--training-logs"]:
+        training_logs_fixtures()
     elif sys.argv[1:] == ["--reference-checks"]:
         reference_checks()
     elif sys.argv[1:] == ["--day-markets"]:
