@@ -23,6 +23,7 @@
  *   rlm_handle_terminal   Agent::HandleTerminal + Policy::HandleTerminal   src/rl/agent.cpp:103-109, policy.cpp:79-82
  *   rlm_go_greedy         Agent::GoGreedy                                  src/rl/agent.cpp:76-79
  *   rlm_read_theta        Agent::write_theta (raw double[MEMORY_SIZE])     src/rl/agent.cpp:176-181
+ *   rlm_save / rlm_load   (none: Agent::write_theta is the reference's only persistence) checkpoint and resume a handle
  *   rlm_eval_q            Agent::getQ / DoubleAgent::getQb on any states   src/rl/agent.cpp:117-135,211-230
  *   rlm_set_model_log     the model_log of Agent::HandleTransition          src/rl/agent.cpp:86-101
  *   rlm_get_policy_descr  Policy::descr (training_log's last column)        src/rl/policy.cpp:18,77,117
@@ -298,6 +299,35 @@ int rlm_get_policy_descr(rlm_handle h, double* out);
 /* theta access: policy = env index (independent) or 0 (shared); table 0 = A, 1 = B (double agents). */
 int rlm_read_theta(rlm_handle h, int32_t policy, int32_t table, double* out, int64_t n);
 int rlm_write_theta(rlm_handle h, int32_t policy, int32_t table, const double* in, int64_t n);
+
+/* ---- checkpoints: save a handle and resume it bit for bit ----------------------------------------------------------
+ * rlm_save waits for the handle's work and writes one file holding every piece of state that carries from one call to the
+ * next: the env records (books, window rings, flow state, agent block), every weight table, the occupancy bitmaps, the
+ * shared-policy dtheta, the trace lists, the generators (mt19937_64, glibc rand and flow state), counters, records, the
+ * model_log state and rows, the tape cursors, day assignment and day markets, the alpha / eps / tau schedules, greedy and
+ * backtest mode, the flow parameters and the engines' run sequence.  rlm_load puts that state into a handle created with
+ * the same rlm_config (every field but `device` and `flow`, which comes from the file), after which the handle continues
+ * as if it had never stopped: the same ticks give bitwise the same weights, records, statistics, counters and logs as the
+ * handle that was saved.  The engine and kernel switches (RLM_ROUNDS, RLM_ENV_VARIANT, RLM_AGENT_VARIANT, RLM_GRAPHS, ...)
+ * may differ between the two handles.
+ * - A save is valid between any two calls: mid-episode or in warm-up, between rlm_handle_terminal and rlm_reset, in
+ *   backtest mode, between the split-surface calls, and between rlm_shared_tick_accumulate and rlm_apply_dtheta (dtheta
+ *   is saved).  A save does not change the handle.
+ * - Weight tables are packed: a bitmap of the 64-bit words that are not +0.0 (bitwise: -0.0 and NaN payloads are kept),
+ *   (memory_size + 7) / 8 bytes, then those words.  Packing and unpacking run on the device in bounded chunks, so only
+ *   the nonzero words cross PCIe and device memory does not grow with n_envs x memory_size.
+ * - Tape handles: the messages are not saved.  The loading handle must hold the same day library (rlm_load_days): the
+ *   file keeps the day offsets and a 64-bit fingerprint of the library's bytes, both checked.
+ * - Stream handles: saved only when every uploaded tick has been consumed (else RLM_ERR_INVALID_ARGUMENT); after a load
+ *   nothing is uploaded, and the caller uploads from the next message on.
+ * - RLM_ENGINE=F|f|p: RLM_ERR_UNSUPPORTED, as for the model_log.
+ * - rlm_load returns RLM_ERR_INVALID_ARGUMENT with the handle unchanged for a missing or truncated file, a bad magic or
+ *   layout version, a config or day library that differs, or a packed table whose bitmap does not match its stored value
+ *   count: the header, the section table, the file length and every bitmap are checked before the handle is written.
+ *   An I/O error while writing returns RLM_ERR_RUNTIME and removes the partial file.
+ * Several ranks of one run each save and load their own shard (their own handle and file). */
+int rlm_save(rlm_handle h, const char* path);
+int rlm_load(rlm_handle h, const char* path);
 
 /* Agent::getQ / DoubleAgent::getQb (agent.cpp:117-135, 211-230) on State::newState(vars, .) (state.cpp:45-51).
  * q_out[i][t][a]: query i, table t (0 = A: getQ; 1 = B: getQb, double_q_learn / double_r_learn only), action a < n_actions.

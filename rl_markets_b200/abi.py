@@ -13,6 +13,9 @@ RLM_MAX_BANDS = 32
 RLM_MAX_ACTIONS = 9
 RLM_N_TILINGS = 32
 RLM_EVAL_Q_CHUNK = 1 << 17  # queries per device pass of rlm_eval_q
+# checkpoint files (rlm_save): the model_log capacity and the saved rlm_config sit at fixed offsets of the header
+CKPT_MODEL_LOG_CAP_OFFSET = 40
+CKPT_CONFIG_OFFSET = 48
 
 # enums (include/rlm.h)
 ALGO = {"q_learn": 0, "sarsa": 1, "double_q_learn": 2, "r_learn": 3, "online_r_learn": 4, "double_r_learn": 5}

@@ -16,7 +16,7 @@ EXPORTS = [
     "rlm_last_error", "rlm_abi_version", "rlm_config_default", "rlm_create", "rlm_destroy", "rlm_reset", "rlm_set_mode", "rlm_new_env", "rlm_set_flow",
     "rlm_load_ticks", "rlm_load_days", "rlm_assign_days", "rlm_get_tape_pos", "rlm_set_day_markets", "rlm_run_ticks", "rlm_sync", "rlm_get_counters", "rlm_get_stats", "rlm_get_state",
     "rlm_get_reward", "rlm_get_actions", "rlm_get_rho", "rlm_get_occupancy", "rlm_copy_theta", "rlm_handle_terminal", "rlm_go_greedy", "rlm_read_theta",
-    "rlm_write_theta", "rlm_eval_q", "rlm_set_model_log", "rlm_read_model_log", "rlm_get_policy_descr", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
+    "rlm_write_theta", "rlm_save", "rlm_load", "rlm_eval_q", "rlm_set_model_log", "rlm_read_model_log", "rlm_get_policy_descr", "rlm_read_records", "rlm_device_ptrs", "rlm_shared_tick_accumulate", "rlm_apply_dtheta",
     "rlm_set_stream", "rlm_set_profiling", "rlm_get_kernel_times", "rlm_act", "rlm_env_step", "rlm_agent_update", "rlm_ingest_csv",
     "rlm_flow_generate", "rlm_test_to_ticks", "rlm_test_to_price", "rlm_test_tiles", "rlm_test_learner_tiles", "rlm_test_order",
     "rlm_test_rolling_mean",
@@ -70,6 +70,8 @@ def load():
     L.rlm_go_greedy.argtypes = [C.c_void_p]
     L.rlm_read_theta.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), C.c_int64]
     L.rlm_write_theta.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), C.c_int64]
+    L.rlm_save.argtypes = [C.c_void_p, C.c_char_p]
+    L.rlm_load.argtypes = [C.c_void_p, C.c_char_p]
     L.rlm_eval_q.argtypes = [C.c_void_p, P(C.c_float), P(C.c_int32), C.c_int64, P(C.c_double)]
     L.rlm_set_model_log.argtypes = [C.c_void_p, C.c_int64]
     L.rlm_read_model_log.argtypes = [C.c_void_p, C.c_int32, C.c_int32, P(C.c_double), P(C.c_int32)]
@@ -279,6 +281,22 @@ class BatchedMarket:
         buf = values if isinstance(values, C.Array) and values._type_ is C.c_double else (C.c_double * n).from_buffer_copy(bytes(values))
         assert len(buf) == n, (len(buf), n)
         check(self.L.rlm_write_theta(self.h, policy, table, buf, n))
+
+    # ---- checkpoints (rlm_save / rlm_load)
+    def save(self, path):
+        """Write every piece of this handle's state to one file (rlm_save); load() into a handle of the same config resumes
+        the run bit for bit."""
+        check(self.L.rlm_save(self.h, os.fsencode(path)))
+
+    def load(self, path):
+        """Resume the handle saved in `path` (rlm_load).  The handle must have been created with the same config (device and
+        flow aside) and, on the tape source, hold the same day library.  Takes over the file's flow parameters and model_log
+        capacity."""
+        check(self.L.rlm_load(self.h, os.fsencode(path)))
+        with open(path, "rb") as f:
+            head = f.read(abi.CKPT_CONFIG_OFFSET + C.sizeof(abi.Config))
+        self._mlog_cap = int.from_bytes(head[abi.CKPT_MODEL_LOG_CAP_OFFSET:abi.CKPT_MODEL_LOG_CAP_OFFSET + 8], "little", signed=True)
+        self.cfg.flow = abi.Config.from_buffer_copy(head, abi.CKPT_CONFIG_OFFSET).flow
 
     @property
     def n_tables(self):
