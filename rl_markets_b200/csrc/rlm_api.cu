@@ -5,115 +5,27 @@
 // codes.  There is deliberately NO CPU execution path here: without a CUDA device
 // rlm_create fails with RLM_ERR_NO_DEVICE.
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <math.h>
+#include <stddef.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 #include <algorithm>
-#include <mutex>
-#include <string>
-#include <vector>
 
-#include "rlm.h"
 #include "rlm_flow_tables.h"
 #include "rlm_rndseq.h"
-#include "rlm_kernels.h"
-#include <errno.h>
-#include <fcntl.h>
-#include <limits.h>
-#include <stddef.h>
-#include <stdlib.h>
-#include <sys/stat.h>
-#include <unistd.h>
+#include "rlm_handle.h"
 
 static thread_local std::string g_err;
-static int fail(int code, const std::string& msg) { g_err = msg; return code; }
-int rlm_set_error_(int code, const std::string& msg) { return fail(code, msg); }  // for the host-only translation units
-#define CK(expr)                                                                                      \
-  do {                                                                                                \
-    cudaError_t _e = (expr);                                                                          \
-    if (_e != cudaSuccess) return fail((_e == cudaErrorNoDevice || _e == cudaErrorInsufficientDriver) ? RLM_ERR_NO_DEVICE : RLM_ERR_CUDA, \
-                                       std::string(#expr) + ": " + cudaGetErrorString(_e));          \
-  } while (0)
-
-struct rlm_handle_s {
-  rlm_config cfg;
-  DevParams hp;
-  DevPtrs ptr;
-  DynParams dyn;
-  cudaStream_t stream = nullptr;
-  bool own_stream = true;
-  int n_sms = 132;
-  int engine = 1;        // 1 tick-synchronous (two launches per tick), 0 persistent queue (rlm_run_kernel), 2 fused (warp per env)
-  int n_agent_ctas = 0;  // persistent engine: CTAs in the agent role
-  int env_variant = 0;   // env tick kernel: 0 = warp per env, 1 = thread per env
-  int agent_variant = 4; // learner kernel: 4 = rlm_learn_kernel (one warp per env, round 2), 3 = three warps per env, 1 = round-1 one-warp kernel
-  unsigned* d_qctl = nullptr;  // [4]: q_head, q_tail, env_warps_done, q_done
-  DynParams shared_dyn;
-  bool in_run = false;
-  // optional per-kernel timing (bench.py roofline leg): CUDA events around every launch of a run call
-  bool profile = false;
-  std::vector<cudaEvent_t> ev;
-  double prof_env_ms = 0, prof_agent_ms = 0;
-  long long prof_env_launches = 0, prof_agent_launches = 0;
-  int ready_cap = 0;  // ticks per run call the ready counters can hold
-  int n_policies = 1;
-  size_t env_bytes = 0;
-  // STREAM source: two device chunks; rlm_load_ticks fills the idle one on a copy stream while the kernels of
-  // earlier rlm_run_ticks calls still read the other (upload of chunk k+1 overlaps compute of chunk k)
-  rlm_tick_msg* d_stream[2] = {nullptr, nullptr};
-  size_t stream_cap[2] = {0, 0};  // messages
-  int stream_buf = 0;
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
-  bool consumed_valid[2] = {false, false};
-  int stream_ticks = 0, stream_cursor = 0;
-  // TAPE source: the day library (ptr.tape, ptr.tape_cur, ptr.tape_lo) and its day boundaries on the host
-  std::vector<int64_t> day_off;  // [n_days + 1]; empty until rlm_load_days
-  std::vector<int32_t> env_day;  // [n_envs] the day each env replays
-  // day markets (rlm_set_day_markets): the market of each day (empty: every day runs under the config's), each env's current
-  // market (-1: the config's; mirrors ptr.env_market, which exists once day markets were first set) and the config's
-  // VenueD, whose IsOpen bounds the uploaded copy gives up while day markets are on (see day_markets_on)
-  std::vector<int32_t> day_market;
-  std::vector<int32_t> env_mkt;
-  int n_markets = 0;  // entries of dm.markets
-  VenueD cfg_venue;
-  DevMarkets dm = {};  // uploaded with hp (rlm_env.cuh: PM)
-  bool rec_dirty = false;  // learner work was enqueued since rlm_fix_terminal_kernel last ran (fix_records)
-  void* d_gather = nullptr; void* h_gather = nullptr; size_t gather_cap = 0;  // rlm_get_reward/actions/state staging
-  long long launches = 0;
-  double alpha = 0, eps = 0, tau = 1.0;
-  // tick-synchronous engine: the batch is cut into n_sub sub-batches, each ticking on its own stream, so that the
-  // DRAM-bound gather burst of one sub-batch's learner kernel overlaps the issue-bound scalar tick kernel of another
-  int n_sub = 1;
-  // CUDA graphs of the tick-synchronous engine (generator source, one stream): one instantiated graph per chunk length,
-  // valid as long as the per-launch parameters it was captured with are unchanged
-  struct TickGraph { int chunk; DynParams d; cudaGraphExec_t exec; };
-  std::vector<TickGraph> graphs;
-  bool use_graphs = true, graph_warm = false;
-  bool staged = false;  // learner: whole-table staging (memory_size * 8 <= 64 KB, independent single-table policies)
-  cudaStream_t sub_stream[RLM_MAX_SUB] = {};
-  cudaEvent_t ev_fork = nullptr, ev_join[RLM_MAX_SUB] = {};
-  // round-paced engine (independent policies, warp-per-env ticks): see run_rounds
-  bool rounds = false;       // forced (RLM_ROUNDS=1)
-  bool in_rounds = false;    // run_rounds is enqueueing (learner launches see more steps)
-  bool rounds_auto = false;  // default: run calls of at least RLM_ROUNDS_MIN_TICKS ticks
-  int run_seq = 0;
-  int round_streams = 1;  // sub-batches of the round-paced engine, each on its own stream (RLM_ROUND_STREAMS)
-  int* h_live = nullptr;  // pinned [RLM_MAX_SUB][2]: ready count of the last round of each group in flight
-  cudaEvent_t ev_live[RLM_MAX_SUB][2] = {};
-  long long rounds_launched = 0, rounds_calls = 0;
-  // model_log (rlm_set_model_log): off while mlog.cap == 0; then one rlm_model_log_kernel pass follows every training
-  // learner launch
-  ModelLogPtrs mlog = {};
-};
+int fail(int code, const std::string& msg) { g_err = msg; return code; }
 
 // The kernels read their per-handle constants from ONE __constant__ block (rlm_env.cuh: P).  g_params_owner says whose
 // they are; another handle takes the block over only after everything launched so far has finished (device-wide
 // synchronisation), and every entry point that launches kernels holds g_api_mu while it does so -- so two handles on
 // one GPU, from one or several host threads, are safe; alternating between them costs a device synchronisation per switch.
 static const rlm_handle_s* g_params_owner = nullptr;
-static std::recursive_mutex g_api_mu;
-#define API_LOCK std::lock_guard<std::recursive_mutex> api_lock_(g_api_mu)
+std::recursive_mutex g_api_mu;
 
 // pinned + device staging area for per-env columns (grown on demand)
 static int split_scratch(rlm_handle_s* h, size_t bytes) {
@@ -127,8 +39,27 @@ static int split_scratch(rlm_handle_s* h, size_t bytes) {
   }
   return RLM_OK;
 }
+// the tail of a staged read-back: the first `bytes` of d_gather, written by the kernels just enqueued, through the pinned
+// staging area (left there for the caller when out is null)
+static int read_back(rlm_handle_s* h, size_t bytes, void* out) {
+  CK(cudaMemcpyAsync(h->h_gather, h->d_gather, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  if (out) memcpy(out, h->h_gather, bytes);
+  return RLM_OK;
+}
 
-extern "C" {
+// The DynParams of a launch of n_ticks ticks: the handle's switches and modes with its current alpha / epsilon / tau.
+static DynParams launch_dyn(rlm_handle_s* h, int n_ticks) {
+  DynParams d = h->dyn;
+  d.alpha = h->alpha; d.eps = h->eps; d.tau = h->tau; d.n_ticks = n_ticks;
+  return d;
+}
+
+// The cached CUDA graphs capture the handle's buffers and kernel variants: every change of either drops them.
+void drop_graphs(rlm_handle h) {
+  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
+  h->graphs.clear();
+}
 
 const char* rlm_last_error(void) { return g_err.c_str(); }
 int rlm_abi_version(void) { return RLM_ABI_VERSION; }
@@ -307,9 +238,6 @@ static cudaError_t launch_agent_on(rlm_handle_s* h, const DevPtrs& ptr, const Dy
     return rlm_launch_agent3(ptr, d, n, h->hp.is_double, h->hp.occ_smem_words, tslot, h->n_sms, stage, full, st);
   }
   return rlm_launch_agent(ptr, d, n, h->hp.scratch_bytes, tslot, h->n_sms, stage, st);
-}
-static cudaError_t launch_agent_any(rlm_handle_s* h, const DynParams& d, int tslot, int stage) {
-  return launch_agent_on(h, h->ptr, d, tslot, stage, h->stream);
 }
 // model_log: the accumulation pass over envs env0 .. env0+n-1 after a learner launch of training (HandleTransition's
 // _agg_delta / _update_counter).  Nothing is launched while the log is off or in backtest mode (Backtester::_step never
@@ -507,11 +435,7 @@ static int create_impl(const rlm_config* cfg, rlm_handle_s* h) {
     }
     if (!getenv("RLM_ROUND_CAP")) h->dyn.round_cap = 3;
     if (const char* s = getenv("RLM_PDL")) rlm_set_pdl(atoi(s));  // programmatic dependent launch of the per-tick kernels (default off: slower when measured)
-    if (const char* s = getenv("RLM_AGENT_VARIANT")) { const int v = atoi(s); h->agent_variant = (v == 1 || v == 3) ? v : 4; }
-    if (cfg->memory_size > (1LL << 27)) {  // (packed tile table of the one-warp learner step, also inside the fused engine)
-      if (h->agent_variant == 4) h->agent_variant = 3;
-      if (h->engine == 3) h->engine = 1;
-    }
+    if (cfg->memory_size > (1LL << 27) && h->engine == 3) h->engine = 1;  // (the packed tile table, inside the fused engine too)
   }
   if (cfg->source == RLM_SOURCE_TAPE) {
     if (h->engine != 1) return fail(RLM_ERR_UNSUPPORTED, "the tape source runs on the tick-synchronous and round-paced engines (RLM_ENGINE=F|f|p read the stream source only)");
@@ -548,7 +472,7 @@ int rlm_destroy(rlm_handle h) {
   cudaFree(h->ptr.q_slots); cudaFree(h->ptr.ag_done); cudaFree(h->d_qctl);
   cudaFree(h->mlog.acc); cudaFree(h->mlog.written); cudaFree(h->mlog.rows);
   for (auto e : h->ev) cudaEventDestroy(e);
-  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
+  drop_graphs(h);
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   for (int s = 0; s < RLM_MAX_SUB; ++s) {
     if (h->sub_stream[s]) { cudaStreamSynchronize(h->sub_stream[s]); cudaStreamDestroy(h->sub_stream[s]); }
@@ -670,7 +594,7 @@ int rlm_load_ticks(rlm_handle h, const rlm_tick_msg* msgs, int32_t n_ticks) {
 }
 
 // ---- TAPE source -------------------------------------------------------------------------------------------------
-static int tape_check(rlm_handle h) {
+int tape_check(rlm_handle h) {
   if (h->cfg.source == RLM_SOURCE_TAPE && h->day_off.empty()) return fail(RLM_ERR_INVALID_ARGUMENT, "no day library loaded (rlm_load_days)");
   return RLM_OK;
 }
@@ -678,14 +602,14 @@ static int tape_check(rlm_handle h) {
 // terminal flag from it (fill_record).  That copy is made to never close, so the flag they write is the date change of
 // Intraday::isTerminal alone, and rlm_fix_terminal_kernel adds the close of the env's own market.  The tick kernels read
 // every env's market from ptr.markets (the MKT instantiations), so nothing else reads the constant copy's hours.
-static void day_markets_on(rlm_handle h, bool on) {
+void day_markets_on(rlm_handle h, bool on) {
   h->hp.venue = h->cfg_venue;
   if (on) { h->hp.venue.open_lo = LLONG_MIN; h->hp.venue.close_hi = LLONG_MAX; }
   g_params_owner = nullptr;  // upload again
 }
 // the records written since the last call get the close of their env's current market (day markets on, params uploaded;
 // nothing to do unless learner work was enqueued since)
-static int fix_records(rlm_handle h) {
+int fix_records(rlm_handle h) {
   if (!h->dm.markets || h->hp.record_envs <= 0 || !h->rec_dirty) return RLM_OK;
   int rc = upload_params(h);
   if (rc) return rc;
@@ -760,9 +684,7 @@ int rlm_load_days(rlm_handle h, const rlm_tick_msg* msgs, const int64_t* day_off
     h->n_markets = 0;
     day_markets_on(h, false);
   }
-  // the cached CUDA graphs hold the old library's address (DevPtrs is captured by value)
-  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
-  h->graphs.clear();
+  drop_graphs(h);  // (they hold the old library's address: DevPtrs is captured by value)
   cudaFree((void*)h->ptr.tape);
   h->ptr.tape = nullptr;
   h->day_off.clear();
@@ -835,9 +757,7 @@ int rlm_set_day_markets(rlm_handle h, const rlm_market* markets, int32_t n_marke
   h->n_markets = n_markets;
   h->day_market.assign(day_market, day_market + n_days);
   day_markets_on(h, true);
-  // the cached CUDA graphs hold the tick kernels without day markets
-  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
-  h->graphs.clear();
+  drop_graphs(h);  // (they hold the tick kernels without day markets)
   // every env back to the start of its day, now under the day's market
   std::vector<int32_t> day(h->env_day);
   return tape_assign(h, 0, h->cfg.n_envs, day.data(), true);
@@ -860,6 +780,8 @@ int rlm_get_tape_pos(rlm_handle h, int64_t* out) {
 
 static int run_ticks_impl(rlm_handle h, int32_t n_ticks);
 static int run_rounds(rlm_handle h, const DynParams& d, int n_ticks);
+static int shared_accumulate(rlm_handle h, const DynParams& d);
+static int shared_apply(rlm_handle h);
 #define RLM_ROUNDS_MIN_TICKS 128
 
 int rlm_run_ticks(rlm_handle h, int32_t n_ticks) {
@@ -875,6 +797,101 @@ int rlm_run_ticks(rlm_handle h, int32_t n_ticks) {
     h->consumed_valid[h->stream_buf] = true;
   }
   return rc;
+}
+
+// Sub-batch s of S holds envs sub0[s] .. sub0[s + 1] - 1: whole warps of the thread-per-env kernel, whole CTAs of the
+// warp-per-env one.
+static void split_batch(int B, int S, int* sub0) {
+  const int per = (((B + S - 1) / S) + 31) & ~31;
+  for (int s = 0; s <= S; ++s) sub0[s] = std::min(B, s * per);
+}
+
+// *out = the cached graph of (chunk, d), on a miss captured on st from enqueue(st, &kernels it launches).  A full cache (cap
+// graphs) is dropped first, after a sync of the handle's stream if sync_drop; *dropped: the graphs had before are gone.
+template <class Enqueue>
+static int cached_graph(rlm_handle h, int chunk, const DynParams& d, size_t cap, bool sync_drop, cudaStream_t st, Enqueue enqueue,
+                        rlm_handle_s::TickGraph* out, bool* dropped = nullptr) {
+  if (dropped) *dropped = false;
+  for (const auto& g : h->graphs)
+    if (g.chunk == chunk && memcmp(&g.d, &d, sizeof(DynParams)) == 0) { *out = g; return RLM_OK; }
+  if (h->graphs.size() >= cap) {
+    if (sync_drop) CK(cudaStreamSynchronize(h->stream));
+    drop_graphs(h);
+    if (dropped) *dropped = true;
+  }
+  rlm_handle_s::TickGraph g = {chunk, d, nullptr, 0};
+  cudaGraph_t graph = nullptr;
+  CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  const int rc = enqueue(st, &g.launches);
+  cudaError_t ce = cudaStreamEndCapture(st, &graph);
+  if (rc == RLM_OK && ce == cudaSuccess) ce = cudaGraphInstantiate(&g.exec, graph, 0);
+  if (graph) cudaGraphDestroy(graph);
+  if (rc != RLM_OK) return rc;
+  CK(ce);
+  h->graphs.push_back(g);
+  *out = g;
+  return RLM_OK;
+}
+
+// Bench instrumentation (rlm_set_profiling, which turns the graphs off): event i of a direct call, 3 per tick or round
+static cudaError_t prof_mark(rlm_handle h, int i, cudaStream_t st) {
+  if (!h->profile) return cudaSuccess;
+  while ((int)h->ev.size() <= i) {
+    cudaEvent_t e;
+    const cudaError_t ce = cudaEventCreate(&e);
+    if (ce != cudaSuccess) return ce;
+    h->ev.push_back(e);
+  }
+  return cudaEventRecord(h->ev[i], st);
+}
+// ... and the kernel times of n ticks or rounds once st has run them: every launch counts, or (ready_count: a round
+// group's counters) only the kernels of the rounds that had work
+static cudaError_t prof_collect(rlm_handle h, int n, cudaStream_t st, const int* ready_count) {
+  std::vector<int> cnt(2 * n, 1);  // [n] envs ready, then [n] envs live
+  cudaError_t ce = cudaStreamSynchronize(st);
+  if (ce == cudaSuccess && ready_count) ce = cudaMemcpy(cnt.data(), ready_count, (size_t)n * 4, cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && ready_count) ce = cudaMemcpy(cnt.data() + n, ready_count + RLM_LIVE_OFF, (size_t)n * 4, cudaMemcpyDeviceToHost);
+  for (int i = 0; i < n && ce == cudaSuccess; ++i) {
+    float a = 0, b = 0;
+    ce = cudaEventElapsedTime(&a, h->ev[3 * i], h->ev[3 * i + 1]);
+    if (ce == cudaSuccess) ce = cudaEventElapsedTime(&b, h->ev[3 * i + 1], h->ev[3 * i + 2]);
+    if (cnt[n + i] > 0) { h->prof_env_ms += a; h->prof_env_launches++; }
+    if (cnt[i] > 0) { h->prof_agent_ms += b; h->prof_agent_launches++; }
+  }
+  return ce;
+}
+
+// One chunk of the tick-synchronous engine on st, captured into a graph or launched directly: the chunk's ready counters
+// cleared, then every tick's env, learner and model_log kernels; *launched counts the kernels.
+static int enqueue_ticks(rlm_handle h, const DevPtrs& ps, const DynParams& dt, int chunk, cudaStream_t st, long long* launched) {
+  CK(cudaMemsetAsync(ps.ready_count, 0, (size_t)chunk * 4, st));
+  for (int t = 0; t < chunk; ++t) {
+    CK(prof_mark(h, 3 * t, st));
+    CK(rlm_launch_env(ps, dt, h->cfg.n_envs, t, 0, h->env_variant, st));
+    CK(prof_mark(h, 3 * t + 1, st));
+    CK(launch_agent_on(h, ps, dt, t, 0, st));
+    CK(prof_mark(h, 3 * t + 2, st));
+    *launched += 2;
+    CK(model_log_pass(h, dt, dt.env0, dt.n_sub, st, launched));
+  }
+  return RLM_OK;
+}
+
+// One group of G rounds of the round-paced engine on st, captured into a graph or launched directly: the group's ready and
+// live counters cleared, then every round's env, learner and model_log kernels; *launched counts the kernels.
+static int enqueue_rounds(rlm_handle h, const DevPtrs& ps, const DynParams& dt, int G, cudaStream_t st, long long* launched) {
+  CK(cudaMemsetAsync(ps.ready_count, 0, (size_t)G * 4, st));
+  CK(cudaMemsetAsync(ps.ready_count + RLM_LIVE_OFF, 0, (size_t)G * 4, st));
+  for (int r = 0; r < G; ++r) {
+    CK(prof_mark(h, 3 * r, st));
+    CK(rlm_launch_env_round(ps, dt, dt.n_sub, r, st));
+    CK(prof_mark(h, 3 * r + 1, st));
+    CK(launch_agent_on(h, ps, dt, r, 0, st));
+    CK(prof_mark(h, 3 * r + 2, st));
+    *launched += 2;
+    CK(model_log_pass(h, dt, dt.env0, dt.n_sub, st, launched));
+  }
+  return RLM_OK;
 }
 
 // Round-paced engine.  A round = rlm_env_round_kernel (every live env ticks until its step ends or its n_ticks are used
@@ -893,25 +910,20 @@ static int run_rounds(rlm_handle h, const DynParams& d, int n_ticks) {
 }
 static int run_rounds_impl(rlm_handle h, const DynParams& d, int n_ticks) {
   const int B = h->cfg.n_envs;
-  RunCtl rc = {++h->run_seq, n_ticks, d.stream_off, d.stream_ticks, h->ptr.stream, 0};
-  CK(rlm_launch_runctl(h->ptr, rc, h->stream));
+  const RunCtl ctl = {++h->run_seq, n_ticks, d.stream_off, d.stream_ticks, h->ptr.stream, 0};
+  CK(rlm_launch_runctl(h->ptr, ctl, h->stream));
   // sub-batches on their own streams: the learner kernel of one (throughput-bound: more steps than resident warps)
   // runs while the tick kernel of another (latency-bound: a few serial ticks per env) does
   const int S = h->profile ? 1 : std::max(1, std::min(h->round_streams, (B + 255) / 256));
   int sub0[RLM_MAX_SUB + 1];
-  {
-    const int per = (((B + S - 1) / S) + 31) & ~31;
-    for (int s = 0; s <= S; ++s) sub0[s] = std::min(B, s * per);
-  }
+  split_batch(B, S, sub0);
   int G = n_ticks >= 512 ? 32 : (n_ticks >= 128 ? 16 : 8);
   G = std::min(std::min(G, n_ticks + 1), h->ready_cap);
   const bool graphs = h->use_graphs && h->graph_warm && !h->profile;
   h->graph_warm = true;  // (the first call launches directly: function attributes are set outside any capture)
-  if (h->profile) while ((int)h->ev.size() < 3 * G) { cudaEvent_t e; CK(cudaEventCreate(&e)); h->ev.push_back(e); }
   DynParams dts[RLM_MAX_SUB];
   DevPtrs pss[RLM_MAX_SUB];
-  cudaGraphExec_t exec[RLM_MAX_SUB] = {};
-  long long ml_captured = 0;  // (a graph's model_log passes are counted when it is launched)
+  rlm_handle_s::TickGraph gs[RLM_MAX_SUB] = {};  // exec null: the sub-batch's groups launch directly
   if (S > 1) CK(cudaEventRecord(h->ev_fork, h->stream));
   for (int s = 0; s < S; ++s) {
     cudaStream_t st = S > 1 ? h->sub_stream[s] : h->stream;
@@ -925,70 +937,29 @@ static int run_rounds_impl(rlm_handle h, const DynParams& d, int n_ticks) {
     ps.ready = h->ptr.ready + sub0[s];
     ps.ready_count = h->ptr.ready_count + (size_t)s * h->ready_cap;
     if (!graphs || dt.n_sub <= 0) continue;
-    for (auto& g : h->graphs)
-      if (g.chunk == -G && memcmp(&g.d, &dt, sizeof(DynParams)) == 0) exec[s] = g.exec;
-    if (!exec[s]) {
-      if (h->graphs.size() >= 24) {
-        CK(cudaStreamSynchronize(h->stream));
-        for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
-        h->graphs.clear();
-        for (int q = 0; q < s; ++q) exec[q] = nullptr;  // (re-captured below when launched directly this call)
-      }
-      cudaGraph_t graph = nullptr;
-      CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      cudaError_t ce = cudaMemsetAsync(ps.ready_count, 0, (size_t)G * 4, st);
-      if (ce == cudaSuccess) ce = cudaMemsetAsync(ps.ready_count + RLM_LIVE_OFF, 0, (size_t)G * 4, st);
-      for (int r = 0; r < G && ce == cudaSuccess; ++r) {
-        ce = rlm_launch_env_round(ps, dt, dt.n_sub, r, st);
-        if (ce == cudaSuccess) ce = launch_agent_on(h, ps, dt, r, 0, st);
-        if (ce == cudaSuccess) ce = model_log_pass(h, dt, dt.env0, dt.n_sub, st, &ml_captured);
-      }
-      cudaError_t ce2 = cudaStreamEndCapture(st, &graph);
-      if (ce != cudaSuccess || ce2 != cudaSuccess) { if (graph) cudaGraphDestroy(graph); CK(ce != cudaSuccess ? ce : ce2); }
-      ce = cudaGraphInstantiate(&exec[s], graph, 0);
-      cudaGraphDestroy(graph);
-      CK(ce);
-      h->graphs.push_back({-G, dt, exec[s]});
-    }
+    bool dropped = false;
+    const int rc = cached_graph(h, -G, dt, 24, true, st,
+                                [&](cudaStream_t cs, long long* n) { return enqueue_rounds(h, ps, dt, G, cs, n); }, &gs[s], &dropped);
+    if (rc) return rc;
+    if (dropped)
+      for (int q = 0; q < s; ++q) gs[q].exec = nullptr;
   }
   const int max_groups = (n_ticks + 1 + G - 1) / G + 1;  // a round advances every live env by at least one tick
   bool live[RLM_MAX_SUB];
   int n_live = 0;
   for (int s = 0; s < S; ++s) { live[s] = sub0[s + 1] > sub0[s]; n_live += live[s] ? 1 : 0; }
-  h->rounds_calls++;
   for (int k = 0; k <= max_groups && n_live > 0; ++k) {
     for (int s = 0; s < S && k < max_groups; ++s) {
       if (!live[s]) continue;
       cudaStream_t st = S > 1 ? h->sub_stream[s] : h->stream;
-      if (exec[s]) CK(cudaGraphLaunch(exec[s], st));
-      else {
-        CK(cudaMemsetAsync(pss[s].ready_count, 0, (size_t)G * 4, st));
-        CK(cudaMemsetAsync(pss[s].ready_count + RLM_LIVE_OFF, 0, (size_t)G * 4, st));
-        for (int r = 0; r < G; ++r) {
-          if (h->profile) CK(cudaEventRecord(h->ev[3 * r], st));
-          CK(rlm_launch_env_round(pss[s], dts[s], dts[s].n_sub, r, st));
-          if (h->profile) CK(cudaEventRecord(h->ev[3 * r + 1], st));
-          CK(launch_agent_on(h, pss[s], dts[s], r, 0, st));
-          if (h->profile) CK(cudaEventRecord(h->ev[3 * r + 2], st));
-          CK(model_log_pass(h, dts[s], dts[s].env0, dts[s].n_sub, st, &h->launches));
-        }
-        if (h->profile) {  // bench instrumentation: per-kernel times of the rounds that had work (S == 1, direct launches)
-          std::vector<int> cnt(2 * G);
-          CK(cudaStreamSynchronize(st));
-          CK(cudaMemcpy(cnt.data(), pss[s].ready_count, (size_t)G * 4, cudaMemcpyDeviceToHost));
-          CK(cudaMemcpy(cnt.data() + G, pss[s].ready_count + RLM_LIVE_OFF, (size_t)G * 4, cudaMemcpyDeviceToHost));
-          for (int r = 0; r < G; ++r) {
-            float a = 0, b = 0;
-            CK(cudaEventElapsedTime(&a, h->ev[3 * r], h->ev[3 * r + 1]));
-            CK(cudaEventElapsedTime(&b, h->ev[3 * r + 1], h->ev[3 * r + 2]));
-            if (cnt[G + r] > 0) { h->prof_env_ms += a; h->prof_env_launches++; }
-            if (cnt[r] > 0) { h->prof_agent_ms += b; h->prof_agent_launches++; }
-          }
-        }
+      if (gs[s].exec) {
+        CK(cudaGraphLaunch(gs[s].exec, st));
+        h->launches += gs[s].launches;
+      } else {
+        const int rc = enqueue_rounds(h, pss[s], dts[s], G, st, &h->launches);
+        if (rc) return rc;
+        if (h->profile) CK(prof_collect(h, G, st, pss[s].ready_count));  // (S == 1)
       }
-      h->launches += 2 * G;
-      if (exec[s]) h->launches += h->mlog.cap > 0 ? G : 0;  // (the graph's model_log passes)
-      h->rounds_launched += G;
       CK(cudaMemcpyAsync(h->h_live + 2 * s + (k & 1), pss[s].ready_count + RLM_LIVE_OFF + (G - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
       CK(cudaEventRecord(h->ev_live[s][k & 1], st));
     }
@@ -1013,8 +984,7 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
   if (rc) return rc;
   rc = upload_params(h);
   if (rc) return rc;
-  DynParams d = h->dyn;
-  d.alpha = h->alpha; d.eps = h->eps; d.tau = h->tau; d.n_ticks = n_ticks;
+  DynParams d = launch_dyn(h, n_ticks);
   if (h->cfg.source == RLM_SOURCE_STREAM) {
     if (h->stream_cursor + n_ticks > h->stream_ticks)
       return fail(RLM_ERR_END_OF_DATA, "rlm_run_ticks: not enough ticks loaded (performAction would return false, base.cpp:289)");
@@ -1025,16 +995,13 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
   if (h->cfg.shared_policy && !d.backtest) {
     // single-GPU shared policy: every tick = accumulate, apply (no all-reduce needed).  Evaluation (backtest mode) never
     // writes theta, so it needs neither stage: it takes the tick-synchronous path below with every env reading policy 0.
-    const DynParams keep = h->dyn;
-    h->in_run = true;
     for (int t = 0; t < n_ticks; ++t) {
-      h->dyn = keep; h->dyn.stream_off = d.stream_off + t; h->dyn.stream_ticks = d.stream_ticks;
-      int rc2 = rlm_shared_tick_accumulate(h);
-      if (!rc2) rc2 = rlm_apply_dtheta(h);
-      if (rc2) { h->dyn = keep; h->in_run = false; return rc2; }
+      DynParams dt = d;
+      dt.n_ticks = 1; dt.stream_off = d.stream_off + t;
+      rc = shared_accumulate(h, dt);
+      if (!rc) rc = shared_apply(h);
+      if (rc) return rc;
     }
-    h->dyn = keep;
-    h->in_run = false;
     return RLM_OK;
   }
   if (h->engine == 2) {
@@ -1064,72 +1031,39 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
   const int S = (h->profile || h->n_sub < 1) ? 1 : h->n_sub;
   const int B = h->cfg.n_envs;
   int sub0[RLM_MAX_SUB + 1];
-  {
-    const int per = (((B + S - 1) / S) + 31) & ~31;  // whole warps of the thread-per-env kernel, whole CTAs of the warp-per-env one
-    for (int s = 0; s <= S; ++s) sub0[s] = std::min(B, s * per);
-  }
+  split_batch(B, S, sub0);
   if (S > 1) {
     CK(cudaEventRecord(h->ev_fork, h->stream));
     for (int s = 0; s < S; ++s) CK(cudaStreamWaitEvent(h->sub_stream[s], h->ev_fork, 0));
   }
-  int done = 0;
   // One CUDA graph per chunk instead of 2 * chunk launches: every node's parameters are fixed (the generator source has
   // no stream offset), so the instantiated graph is reused until alpha / epsilon / the mode change.
   const bool graphs = h->use_graphs && h->graph_warm && S == 1 && !h->profile;
   const bool from_stream = h->cfg.source == RLM_SOURCE_STREAM;
   h->graph_warm = true;  // (the first call launches directly: function attributes are set outside any capture)
-  while (graphs && done < n_ticks) {
+  for (int done = 0; done < n_ticks;) {
     const int chunk = std::min(n_ticks - done, h->ready_cap);
-    DynParams dt = d;
-    dt.env0 = 0; dt.n_sub = B; dt.sub_idx = 0;
-    DevPtrs pg = h->ptr;
-    if (from_stream) {
-      // STREAM source: what changes from call to call (buffer, offset, length) goes through device memory, so that the
-      // graph of a chunk is reused by every call -- and by both buffers of the double-buffered upload
-      dt.ctl_stream = 1; dt.stream_off = 0; dt.stream_ticks = 0;
-      pg.stream = nullptr;
-      RunCtl rc = {++h->run_seq, n_ticks, d.stream_off + done, d.stream_ticks, h->ptr.stream, 0};
-      CK(rlm_launch_runctl(h->ptr, rc, h->stream));
-    }
-    rlm_handle_s::TickGraph* tg = nullptr;
-    long long ml_dummy = 0;
-    for (auto& g : h->graphs)
-      if (g.chunk == chunk && memcmp(&g.d, &dt, sizeof(DynParams)) == 0) tg = &g;
-    if (!tg) {
-      if (h->graphs.size() >= 8) { for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec); h->graphs.clear(); }
-      cudaGraph_t graph = nullptr;
-      CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-      cudaError_t ce = cudaMemsetAsync(h->ptr.ready_count, 0, (size_t)chunk * 4, h->stream);
-      for (int t = 0; t < chunk && ce == cudaSuccess; ++t) {
-        ce = rlm_launch_env(pg, dt, B, t, 0, h->env_variant, h->stream);
-        if (ce == cudaSuccess) ce = launch_agent_on(h, pg, dt, t, 0, h->stream);
-        if (ce == cudaSuccess) ce = model_log_pass(h, dt, 0, B, h->stream, &ml_dummy);
+    if (graphs) {
+      DynParams dt = d;
+      dt.env0 = 0; dt.n_sub = B; dt.sub_idx = 0;
+      DevPtrs pg = h->ptr;
+      if (from_stream) {
+        // STREAM source: what changes from call to call (buffer, offset, length) goes through device memory, so that the
+        // graph of a chunk is reused by every call -- and by both buffers of the double-buffered upload
+        dt.ctl_stream = 1; dt.stream_off = 0; dt.stream_ticks = 0;
+        pg.stream = nullptr;
+        const RunCtl ctl = {++h->run_seq, n_ticks, d.stream_off + done, d.stream_ticks, h->ptr.stream, 0};
+        CK(rlm_launch_runctl(h->ptr, ctl, h->stream));
       }
-      cudaError_t ce2 = cudaStreamEndCapture(h->stream, &graph);
-      if (ce != cudaSuccess || ce2 != cudaSuccess) { if (graph) cudaGraphDestroy(graph); CK(ce != cudaSuccess ? ce : ce2); }
-      cudaGraphExec_t exec = nullptr;
-      ce = cudaGraphInstantiate(&exec, graph, 0);
-      cudaGraphDestroy(graph);
-      CK(ce);
-      h->graphs.push_back({chunk, dt, exec});
-      tg = &h->graphs.back();
-    }
-    CK(cudaGraphLaunch(tg->exec, h->stream));
-    h->launches += 2 * chunk;
-    if (h->mlog.cap > 0 && !d.backtest) h->launches += chunk;  // (the graph's model_log passes)
-    done += chunk;
-  }
-  while (done < n_ticks) {
-    const int chunk = std::min(n_ticks - done, h->ready_cap);
-    if (h->profile) {
-      while ((int)h->ev.size() < 3 * chunk) { cudaEvent_t e; CK(cudaEventCreate(&e)); h->ev.push_back(e); }
-    }
-    for (int s = 0; s < S; ++s)
-      CK(cudaMemsetAsync(h->ptr.ready_count + (size_t)s * h->ready_cap, 0, (size_t)chunk * 4, S > 1 ? h->sub_stream[s] : h->stream));
-    for (int t = 0; t < chunk; ++t) {
+      rlm_handle_s::TickGraph g = {};
+      rc = cached_graph(h, chunk, dt, 8, false, h->stream,
+                        [&](cudaStream_t st, long long* n) { return enqueue_ticks(h, pg, dt, chunk, st, n); }, &g);
+      if (rc) return rc;
+      CK(cudaGraphLaunch(g.exec, h->stream));
+      h->launches += g.launches;
+    } else {
       for (int s = 0; s < S; ++s) {
         if (sub0[s + 1] <= sub0[s]) continue;
-        cudaStream_t st = S > 1 ? h->sub_stream[s] : h->stream;
         DynParams dt = d;
         dt.stream_off = d.stream_off + done;
         dt.env0 = sub0[s];
@@ -1138,24 +1072,10 @@ static int run_ticks_impl(rlm_handle h, int32_t n_ticks) {
         DevPtrs ps = h->ptr;
         ps.ready = h->ptr.ready + sub0[s];
         ps.ready_count = h->ptr.ready_count + (size_t)s * h->ready_cap;
-        if (h->profile) CK(cudaEventRecord(h->ev[3 * t], st));
-        CK(rlm_launch_env(ps, dt, B, t, 0, h->env_variant, st));
-        if (h->profile) CK(cudaEventRecord(h->ev[3 * t + 1], st));
-        CK(launch_agent_on(h, ps, dt, t, 0, st));
-        if (h->profile) CK(cudaEventRecord(h->ev[3 * t + 2], st));
-        h->launches += 2;
-        CK(model_log_pass(h, dt, dt.env0, dt.n_sub, st, &h->launches));
+        rc = enqueue_ticks(h, ps, dt, chunk, S > 1 ? h->sub_stream[s] : h->stream, &h->launches);
+        if (rc) return rc;
       }
-    }
-    if (h->profile) {
-      CK(cudaStreamSynchronize(h->stream));
-      for (int t = 0; t < chunk; ++t) {
-        float a = 0, b = 0;
-        CK(cudaEventElapsedTime(&a, h->ev[3 * t], h->ev[3 * t + 1]));
-        CK(cudaEventElapsedTime(&b, h->ev[3 * t + 1], h->ev[3 * t + 2]));
-        h->prof_env_ms += a; h->prof_agent_ms += b;
-        h->prof_env_launches++; h->prof_agent_launches++;
-      }
+      if (h->profile) CK(prof_collect(h, chunk, h->stream, nullptr));  // (S == 1)
     }
     done += chunk;
   }
@@ -1243,20 +1163,10 @@ static int fetch_column(rlm_handle h, int what, void* out, size_t bytes) {
   API_LOCK;
   CK(cudaSetDevice(h->cfg.device));
   int rc = upload_params(h);
+  if (!rc) rc = split_scratch(h, bytes);
   if (rc) return rc;
-  if (bytes > h->gather_cap) {
-    CK(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_gather); if (h->h_gather) cudaFreeHost(h->h_gather);
-    h->d_gather = nullptr; h->h_gather = nullptr; h->gather_cap = 0;
-    CK(cudaMalloc(&h->d_gather, bytes));
-    CK(cudaMallocHost(&h->h_gather, bytes));
-    h->gather_cap = bytes;
-  }
   CK(rlm_launch_gather(h->ptr, h->cfg.n_envs, what, h->d_gather, h->stream));
-  CK(cudaMemcpyAsync(h->h_gather, h->d_gather, bytes, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  memcpy(out, h->h_gather, bytes);
-  return RLM_OK;
+  return read_back(h, bytes, out);
 }
 
 int rlm_get_state(rlm_handle h, float* out) {
@@ -1276,10 +1186,7 @@ int rlm_get_occupancy(rlm_handle h, int32_t* out) {
   int rc = split_scratch(h, bytes);
   if (rc) return rc;
   CK(rlm_launch_count_nonzero(h->ptr.theta, h->cfg.memory_size, h->cfg.n_envs, (int*)h->d_gather, h->stream));
-  CK(cudaMemcpyAsync(h->h_gather, h->d_gather, bytes, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  memcpy(out, h->h_gather, bytes);
-  return RLM_OK;
+  return read_back(h, bytes, out);
 }
 int rlm_get_rho(rlm_handle h, double* out) {
   if (!h || !out) return fail(RLM_ERR_INVALID_ARGUMENT, "null argument");
@@ -1329,9 +1236,7 @@ int rlm_set_model_log(rlm_handle h, int64_t cap_rows) {
       return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_set_model_log: n_envs x cap_rows needs " + std::to_string((long long)(need / 1e6)) +
                                                 " MB of device memory, " + std::to_string((long long)(have / 1e6)) + " MB are free");
   }
-  // the cached CUDA graphs were captured with (or without) the accumulation pass and its buffers
-  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
-  h->graphs.clear();
+  drop_graphs(h);  // (they were captured with, or without, the accumulation pass and its buffers)
   cudaFree(h->mlog.acc); cudaFree(h->mlog.written); cudaFree(h->mlog.rows);
   h->mlog = ModelLogPtrs{};
   if (cap_rows == 0) return RLM_OK;
@@ -1463,9 +1368,8 @@ int rlm_eval_q(rlm_handle h, const float* vars, const int32_t* policy, int64_t n
       dp = (const int*)(d + out_b + var_b);
     }
     CK(rlm_launch_q(h->ptr, dv, dp, vars ? 0 : (int)i0, (int)m, (double*)d, h->hp.is_double, h->n_sms, h->stream));
-    CK(cudaMemcpyAsync(hs, d, (size_t)(m * T * A * 8), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(q_out + i0 * T * A, hs, (size_t)(m * T * A * 8));
+    rc = read_back(h, (size_t)(m * T * A * 8), q_out + i0 * T * A);
+    if (rc) return rc;
   }
   return RLM_OK;
 }
@@ -1529,18 +1433,20 @@ int rlm_shared_tick_accumulate(rlm_handle h) {
   CK(cudaSetDevice(h->cfg.device));
   int rc = upload_params(h);
   if (rc) return rc;
-  DynParams d = h->dyn;
-  d.alpha = h->alpha; d.eps = h->eps; d.tau = h->tau; d.n_ticks = 1;
+  DynParams d = launch_dyn(h, 1);
   rc = tape_check(h);
   if (rc) return rc;
-  if (h->cfg.source == RLM_SOURCE_STREAM && !h->in_run) {
+  if (h->cfg.source == RLM_SOURCE_STREAM) {
     if (h->stream_cursor + 1 > h->stream_ticks) return fail(RLM_ERR_END_OF_DATA, "not enough ticks loaded");
     d.stream_off = h->stream_cursor; d.stream_ticks = h->stream_ticks;
     h->stream_cursor += 1;
   }
+  return shared_accumulate(h, d);
+}
+static int shared_accumulate(rlm_handle h, const DynParams& d) {
   CK(cudaMemsetAsync(h->ptr.ready_count, 0, 4, h->stream));
   CK(rlm_launch_env(h->ptr, d, h->cfg.n_envs, 0, 0, h->env_variant, h->stream));
-  CK(launch_agent_any(h, d, 0, 1));
+  CK(launch_agent_on(h, h->ptr, d, 0, 1, h->stream));
   h->launches += 2;
   h->shared_dyn = d;
   return RLM_OK;
@@ -1555,13 +1461,13 @@ int rlm_apply_dtheta(rlm_handle h) {
   if (h->dyn.backtest) return fail(RLM_ERR_INVALID_ARGUMENT, k_eval_no_collective);
   h->rec_dirty = true;  // (learner steps write records)
   CK(cudaSetDevice(h->cfg.device));
-  int rc = upload_params(h);
-  if (rc) return rc;
-  const long long n =(long long)(h->hp.is_double ? 2 : 1) * h->cfg.memory_size;
+  const int rc = upload_params(h);
+  return rc ? rc : shared_apply(h);
+}
+static int shared_apply(rlm_handle h) {
   CK(rlm_launch_apply_dtheta(h->ptr.theta, h->ptr.dtheta, h->cfg.memory_size, h->n_sms, h->stream));
   if (h->hp.is_double) CK(rlm_launch_apply_dtheta(h->ptr.theta_b, h->ptr.dtheta + h->cfg.memory_size, h->cfg.memory_size, h->n_sms, h->stream));
-  (void)n;
-  CK(launch_agent_any(h, h->shared_dyn, 0, 2));
+  CK(launch_agent_on(h, h->ptr, h->shared_dyn, 0, 2, h->stream));
   CK(rlm_launch_env(h->ptr, h->shared_dyn, h->cfg.n_envs, 0, 1, h->env_variant, h->stream));
   h->launches += 3;
   CK(model_log_pass(h, h->shared_dyn, 0, h->cfg.n_envs, h->stream, &h->launches));
@@ -1582,8 +1488,7 @@ static int split_check(rlm_handle h) {
   return tape_check(h);
 }
 static DynParams split_dyn(rlm_handle h) {
-  DynParams d = h->dyn;
-  d.alpha = h->alpha; d.eps = h->eps; d.tau = h->tau; d.n_ticks = 1;
+  DynParams d = launch_dyn(h, 1);
   d.hold = 1;
   return d;
 }
@@ -1600,11 +1505,8 @@ int rlm_act(rlm_handle h, int32_t* actions_out) {
   rc = split_scratch(h, bytes);
   if (rc) return rc;
   CK(rlm_launch_act(h->ptr, split_dyn(h), h->cfg.n_envs, (int*)h->d_gather, h->stream));
-  CK(cudaMemcpyAsync(h->h_gather, h->d_gather, bytes, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  memcpy(actions_out, h->h_gather, bytes);
   h->launches += 1;
-  return RLM_OK;
+  return read_back(h, bytes, actions_out);
 }
 
 int rlm_env_step(rlm_handle h, const int32_t* actions, double* reward_out, uint8_t* terminal_out) {
@@ -1642,8 +1544,8 @@ int rlm_env_step(rlm_handle h, const int32_t* actions, double* reward_out, uint8
     double* d_rew = (double*)h->d_gather;
     unsigned char* d_term = (unsigned char*)h->d_gather + (size_t)B * 8;
     CK(rlm_launch_step_out(h->ptr, B, d_rew, d_term, nullptr, h->stream));
-    CK(cudaMemcpyAsync(h->h_gather, h->d_gather, (size_t)B * 9, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    rc = read_back(h, (size_t)B * 9, nullptr);
+    if (rc) return rc;
     if (reward_out) memcpy(reward_out, h->h_gather, (size_t)B * 8);
     if (terminal_out) memcpy(terminal_out, (unsigned char*)h->h_gather + (size_t)B * 8, (size_t)B);
   }
@@ -1661,7 +1563,7 @@ int rlm_agent_update(rlm_handle h, double* delta_out) {
   const int B = h->cfg.n_envs;
   // State::newState + Agent::HandleTransition for the envs on the ready list of the last rlm_env_step (backtest mode:
   // State::newState of the next Backtester::_step, the greedy evaluation step)
-  CK(launch_agent_any(h, split_dyn(h), 0, 0));
+  CK(launch_agent_on(h, h->ptr, split_dyn(h), 0, 0, h->stream));
   CK(cudaMemsetAsync(h->ptr.ready_count, 0, 4, h->stream));
   h->launches += 1;
   CK(model_log_pass(h, h->dyn, 0, B, h->stream, &h->launches));
@@ -1672,635 +1574,8 @@ int rlm_agent_update(rlm_handle h, double* delta_out) {
     rc = split_scratch(h, (size_t)B * 8);
     if (rc) return rc;
     CK(rlm_launch_step_out(h->ptr, B, nullptr, nullptr, (double*)h->d_gather, h->stream));
-    CK(cudaMemcpyAsync(h->h_gather, h->d_gather, (size_t)B * 8, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(delta_out, h->h_gather, (size_t)B * 8);
+    return read_back(h, (size_t)B * 8, delta_out);
   }
-  return RLM_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Checkpoints: rlm_save / rlm_load (include/rlm.h).  Everything that carries from one call on a handle to the next, and
-// whether a file holds it:
-//   rlm_handle_s
-//     cfg                  saved; a loading handle must match it field for field except `device`, and takes `flow` from it
-//     hp, cfg_venue        derived from cfg (hp.flow restored with cfg.flow, hp.venue follows the day markets)
-//     dyn                  greedy and backtest saved; the other fields are per-launch values or engine switches
-//     shared_dyn           saved: rlm_apply_dtheta finishes the tick rlm_shared_tick_accumulate began with it
-//     alpha, eps, tau      saved (the schedules of rlm_handle_terminal)
-//     launches             saved
-//     run_seq              saved: the round-paced engine tells its calls apart by EnvHdr::run_id == RunCtl::run_id, so a
-//                          handle restarting at 0 would skip ticks
-//     mlog                 acc, written, rows and cap saved: the log is on in the loaded handle if it was on when saved
-//     day_off              saved, and must equal the loading handle's library (whose bytes are checked by fingerprint)
-//     env_day, day_market, env_mkt, n_markets, dm   saved; dm's buffers are allocated or freed to match
-//     stream_ticks, stream_cursor   equal at a save (every uploaded tick consumed); 0 after a load
-//     d_stream, stream_cap, stream_buf, copy_stream, ev_copied, ev_consumed, consumed_valid   transient: the stream
-//                          source's upload buffers, empty of unconsumed ticks at a save; the caller uploads after a load
-//     rec_dirty            transient: records are fixed (fix_records) before they are saved
-//     stream, own_stream, n_sms, engine, n_agent_ctas, env_variant, agent_variant, n_sub, staged, rounds, rounds_auto,
-//     round_streams, use_graphs   the loading handle's own: its device and stream, and engine switches, under which every
-//                          engine computes the same results
-//     graphs, graph_warm   dropped and cleared by a load (the graphs captured the old buffers and parameters)
-//     d_qctl               transient: persistent engine (RLM_ENGINE=p), which save and load refuse
-//     in_run, in_rounds    transient: false between calls
-//     profile, ev, prof_*, rounds_launched, rounds_calls   transient: measurement hooks
-//     ready_cap, n_policies, env_bytes   derived from cfg
-//     d_gather, h_gather, gather_cap, sub_stream, ev_fork, ev_join, h_live, ev_live   transient: staging and
-//                          synchronisation objects
-//   DevPtrs
-//     env                  saved whole (env_stride bytes per env, window rings included)
-//     theta, theta_b       saved packed, one table per policy
-//     dtheta               saved packed: a save between rlm_shared_tick_accumulate and rlm_apply_dtheta keeps the update
-//     trace_f, trace_e, mt_pol, mt_agt, counters, occ, hsum   saved
-//     records, record_count   saved
-//     ready, ready_count   saved: the ready list of rlm_env_step / rlm_shared_tick_accumulate is read by the next call
-//     tape_cur, tape_lo    saved
-//     tape                 not saved (a library can be gigabytes): the loading handle holds the same one
-//     stream               transient (see d_stream)
-//     runctl               transient: rewritten before every kernel that reads it (round-paced call, stream-source graph)
-//     q_slots, q_head, q_tail, env_warps_done, q_done, ag_done, q_size   transient: persistent engine, refused
-//
-// File: a header (CkHeader), a section table, the raw sections in table order, then every weight table packed -- a
-// bitmap of its words that are not +0.0, (M + 7) / 8 bytes, then those words in index order.  Tables cross PCIe packed
-// (rlm_checkpoint.cu), in chunks of at most RLM_CK_CHUNK words through two device and two pinned buffers: the copy and
-// the write of chunk k run while chunk k + 1 is packed (loading: the read of chunk k + 1 while chunk k is copied and
-// unpacked), so device memory does not grow with n_envs x memory_size.
-#define RLM_CK_VERSION 1
-#define RLM_CK_CHUNK (1LL << 22)
-#define RLM_CK_MAX_TABLES 4096
-
-struct CkHeader {
-  char magic[8];  // "RLMCKPT"
-  uint32_t version, n_sections;
-  uint64_t file_bytes;
-  uint32_t header_bytes;  // header + section table: the first section's offset
-  uint32_t env_stride, env_hdr_bytes, pad;
-  int64_t model_log_cap;  // (offset 40, and the config at 48: rl_markets_b200/lib.py reads both)
-  rlm_config cfg;
-  double alpha, eps, tau;
-  int64_t launches;
-  int32_t run_seq, greedy, backtest, n_days, n_markets, has_env_market;
-  uint64_t library_fp;  // tape: fingerprint of the day library's bytes (rlm_fingerprint_kernel)
-  DynParams shared_dyn;
-};
-static_assert(offsetof(CkHeader, model_log_cap) == 40 && offsetof(CkHeader, cfg) == 48, "lib.py reads the header at fixed offsets");
-struct CkSection { uint32_t id, table; uint64_t offset, bytes, count; };  // count: values of a packed table
-enum { CK_ENV = 1, CK_HSUM, CK_OCC, CK_TRACE_F, CK_TRACE_E, CK_MT_POL, CK_MT_AGT, CK_COUNTERS, CK_READY, CK_READY_COUNT, CK_RECORDS,
-       CK_RECORD_COUNT, CK_TAPE_CUR, CK_TAPE_LO, CK_ENV_DAY, CK_DAY_OFF, CK_DAY_MARKET, CK_MARKETS, CK_ENV_MARKET, CK_REC_FIXED,
-       CK_MLOG_ACC, CK_MLOG_WRITTEN, CK_MLOG_ROWS, CK_THETA = 64, CK_THETA_B, CK_DTHETA };
-
-// what decides the layout beyond the config, and where the sections of a file come from or go to
-struct CkView {
-  long long mlog_cap;
-  int n_days, n_markets, has_env_market;
-  ModelLogPtrs mlog;
-  VenueD* markets;
-  int* rec_fixed;
-  void *env_day, *day_off, *day_market, *env_mkt;  // host sections
-};
-struct CkRaw { uint32_t id; size_t bytes; void* dev; void* host; };
-static std::vector<CkRaw> ck_raw(rlm_handle h, const CkView& v) {
-  const size_t B = h->cfg.n_envs, R = h->hp.record_envs;
-  std::vector<CkRaw> r;
-  auto dev = [&](uint32_t id, size_t bytes, const void* p) { r.push_back({id, bytes, (void*)p, nullptr}); };
-  auto host = [&](uint32_t id, size_t bytes, void* p) { r.push_back({id, bytes, nullptr, p}); };
-  dev(CK_ENV, h->env_bytes, h->ptr.env);
-  dev(CK_HSUM, B * 3 * 32 * 8, h->ptr.hsum);
-  dev(CK_OCC, (size_t)h->n_policies * h->hp.occ_words * 4, h->ptr.occ);
-  dev(CK_TRACE_F, B * h->hp.trace_cap * 4, h->ptr.trace_f);
-  dev(CK_TRACE_E, B * h->hp.trace_cap * 4, h->ptr.trace_e);
-  dev(CK_MT_POL, B * 312 * 8, h->ptr.mt_pol);
-  if (h->ptr.mt_agt) dev(CK_MT_AGT, B * 312 * 8, h->ptr.mt_agt);
-  dev(CK_COUNTERS, 8 * 8, h->ptr.counters);
-  dev(CK_READY, B * 4, h->ptr.ready);
-  dev(CK_READY_COUNT, (size_t)2 * RLM_LIVE_OFF * 4, h->ptr.ready_count);
-  if (R > 0) {
-    dev(CK_RECORDS, R * h->hp.record_cap * sizeof(rlm_step_record), h->ptr.records);
-    dev(CK_RECORD_COUNT, R * 4, h->ptr.record_count);
-  }
-  if (h->cfg.source == RLM_SOURCE_TAPE) {
-    dev(CK_TAPE_CUR, B * sizeof(int2), h->ptr.tape_cur);
-    dev(CK_TAPE_LO, B * 4, h->ptr.tape_lo);
-    host(CK_ENV_DAY, B * 4, v.env_day);
-    host(CK_DAY_OFF, ((size_t)v.n_days + 1) * 8, v.day_off);
-    if (v.n_markets > 0) {
-      host(CK_DAY_MARKET, (size_t)v.n_days * 4, v.day_market);
-      dev(CK_MARKETS, (size_t)v.n_markets * sizeof(VenueD), v.markets);
-    }
-    if (v.has_env_market) {
-      host(CK_ENV_MARKET, B * 4, v.env_mkt);
-      if (R > 0) dev(CK_REC_FIXED, R * 4, v.rec_fixed);
-    }
-  }
-  if (v.mlog_cap > 0) {
-    dev(CK_MLOG_ACC, B * sizeof(ModelLogAcc), v.mlog.acc);
-    dev(CK_MLOG_WRITTEN, B * 8, v.mlog.written);
-    dev(CK_MLOG_ROWS, B * (size_t)v.mlog_cap * 8, v.mlog.rows);
-  }
-  return r;
-}
-static CkView ck_view_of(rlm_handle h) {
-  CkView v = {};
-  v.mlog_cap = h->mlog.cap; v.mlog = h->mlog;
-  v.n_days = h->cfg.source == RLM_SOURCE_TAPE ? (int)h->day_off.size() - 1 : 0;
-  v.n_markets = h->dm.markets ? h->n_markets : 0;
-  v.has_env_market = h->dm.env_market != nullptr;
-  v.markets = (VenueD*)h->dm.markets; v.rec_fixed = h->dm.rec_fixed;
-  v.env_day = h->env_day.data(); v.day_off = h->day_off.data(); v.day_market = h->day_market.data(); v.env_mkt = h->env_mkt.data();
-  return v;
-}
-
-// the weight arrays ([n][M] tables each) and the chunks they are packed in: whole tables, or slices of one table that is
-// larger than a chunk
-struct CkArr { uint32_t id; double* base; int n; };
-struct CkChunk { int arr, t0, nt; long long lo, len; };
-static std::vector<CkArr> ck_arrays(rlm_handle h) {
-  std::vector<CkArr> a;
-  a.push_back({CK_THETA, h->ptr.theta, h->n_policies});
-  if (h->ptr.theta_b) a.push_back({CK_THETA_B, h->ptr.theta_b, h->n_policies});
-  if (h->ptr.dtheta) a.push_back({CK_DTHETA, h->ptr.dtheta, h->hp.is_double ? 2 : 1});
-  return a;
-}
-static std::vector<CkChunk> ck_chunks(const std::vector<CkArr>& arrs, long long M) {
-  std::vector<CkChunk> c;
-  for (int a = 0; a < (int)arrs.size(); ++a) {
-    if (M <= RLM_CK_CHUNK) {
-      const int per = (int)std::min<long long>(RLM_CK_CHUNK / M, RLM_CK_MAX_TABLES);
-      for (int t = 0; t < arrs[a].n; t += per) c.push_back({a, t, std::min(per, arrs[a].n - t), 0, M});
-    } else {
-      for (int t = 0; t < arrs[a].n; ++t)
-        for (long long lo = 0; lo < M; lo += RLM_CK_CHUNK) c.push_back({a, t, 1, lo, std::min(RLM_CK_CHUNK, M - lo)});
-    }
-  }
-  return c;
-}
-static long long ck_bw(long long len) { return (len + 31) / 32; }
-static long long ck_bpt(long long len) { return (len + RLM_CK_TILE - 1) / RLM_CK_TILE; }
-
-// two device and two pinned chunk buffers, the copy stream and the events of the pipeline; freed when it goes out of scope
-struct CkScratch {
-  CkChunkDev d[2] = {};
-  unsigned char* dmem[2] = {};
-  unsigned char* hmem[2] = {};
-  double* h_vals[2] = {};
-  unsigned* h_bits[2] = {};
-  long long* h_cnt[2] = {};
-  long long* h_expect[2] = {};
-  int* h_err = nullptr;
-  unsigned long long* d_fp = nullptr;
-  size_t words = 0, bit_bytes = 0, pinned = 0;
-  cudaStream_t cs = nullptr;
-  cudaEvent_t ev_a[2] = {}, ev_b[2] = {};
-  ~CkScratch() {
-    if (cs) { cudaStreamSynchronize(cs); cudaStreamDestroy(cs); }
-    for (int b = 0; b < 2; ++b) {
-      if (ev_a[b]) cudaEventDestroy(ev_a[b]);
-      if (ev_b[b]) cudaEventDestroy(ev_b[b]);
-      cudaFree(dmem[b]);
-      if (hmem[b]) cudaFreeHost(hmem[b]);
-    }
-    cudaFree(d_fp);
-    if (h_err) cudaFreeHost(h_err);
-  }
-};
-static size_t ck_al(size_t x) { return (x + 255) & ~(size_t)255; }
-static int ck_scratch(rlm_handle h, CkScratch& s, const std::vector<CkChunk>& ch) {
-  size_t words = 1, bits = 1, blocks = 1, nt = 1;
-  for (const CkChunk& c : ch) {
-    words = std::max(words, (size_t)(c.nt * c.len));
-    bits = std::max(bits, (size_t)(c.nt * ck_bw(c.len)));
-    blocks = std::max(blocks, (size_t)(c.nt * ck_bpt(c.len)));
-    nt = std::max(nt, (size_t)c.nt);
-  }
-  s.words = words;
-  s.bit_bytes = bits * 4;
-  const size_t dbytes = ck_al(words * 8) + ck_al(bits * 4) + ck_al(blocks * 4) + ck_al((blocks + 1) * 8) + 2 * ck_al(nt * 8) + 256;
-  s.pinned = ck_al(words * 8) + ck_al(bits * 4) + 2 * ck_al(nt * 8);
-  CK(cudaStreamCreateWithFlags(&s.cs, cudaStreamNonBlocking));
-  CK(cudaMalloc(&s.d_fp, 8));
-  CK(cudaMallocHost(&s.h_err, 2 * sizeof(int)));
-  for (int b = 0; b < 2; ++b) {
-    CK(cudaEventCreateWithFlags(&s.ev_a[b], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&s.ev_b[b], cudaEventDisableTiming));
-    CK(cudaMalloc(&s.dmem[b], dbytes));
-    CK(cudaMallocHost(&s.hmem[b], s.pinned));
-    unsigned char* p = s.dmem[b];
-    s.d[b].vals = (double*)p; p += ck_al(words * 8);
-    s.d[b].bits = (unsigned*)p; p += ck_al(bits * 4);
-    s.d[b].blk_cnt = (int*)p; p += ck_al(blocks * 4);
-    s.d[b].off = (long long*)p; p += ck_al((blocks + 1) * 8);
-    s.d[b].cnt = (long long*)p; p += ck_al(nt * 8);
-    s.d[b].expect = (long long*)p; p += ck_al(nt * 8);
-    s.d[b].err = (int*)p;
-    unsigned char* q = s.hmem[b];
-    s.h_vals[b] = (double*)q; q += ck_al(words * 8);
-    s.h_bits[b] = (unsigned*)q; q += ck_al(bits * 4);
-    s.h_cnt[b] = (long long*)q; q += ck_al(nt * 8);
-    s.h_expect[b] = (long long*)q;
-    CK(cudaMemsetAsync(s.d[b].err, 0, sizeof(int), h->stream));
-  }
-  return RLM_OK;
-}
-
-static bool ck_pwrite(int fd, const void* p, size_t n, uint64_t off) {
-  const char* c = (const char*)p;
-  while (n > 0) {
-    const ssize_t w = pwrite(fd, c, n, (off_t)off);
-    if (w <= 0) return false;
-    c += w; n -= (size_t)w; off += (uint64_t)w;
-  }
-  return true;
-}
-static bool ck_pread(int fd, void* p, size_t n, uint64_t off) {
-  char* c = (char*)p;
-  while (n > 0) {
-    const ssize_t r = pread(fd, c, n, (off_t)off);
-    if (r <= 0) return false;
-    c += r; n -= (size_t)r; off += (uint64_t)r;
-  }
-  return true;
-}
-static int ck_io_fail(const char* what, const char* path) {
-  return fail(RLM_ERR_RUNTIME, std::string(what) + " " + path + ": " + strerror(errno));
-}
-
-// raw device sections pass through pinned buffer 0
-static int ck_raw_save(rlm_handle h, int fd, CkScratch& s, const CkRaw& r, uint64_t off, const char* path) {
-  if (r.host) return ck_pwrite(fd, r.host, r.bytes, off) ? RLM_OK : ck_io_fail("rlm_save: cannot write", path);
-  for (size_t done = 0; done < r.bytes;) {
-    const size_t n = std::min(s.pinned, r.bytes - done);
-    CK(cudaMemcpyAsync(s.hmem[0], (const unsigned char*)r.dev + done, n, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    if (!ck_pwrite(fd, s.hmem[0], n, off + done)) return ck_io_fail("rlm_save: cannot write", path);
-    done += n;
-  }
-  return RLM_OK;
-}
-static int ck_raw_load(rlm_handle h, int fd, CkScratch& s, const CkRaw& r, uint64_t off, const char* path) {
-  for (size_t done = 0; done < r.bytes;) {
-    const size_t n = std::min(s.pinned, r.bytes - done);
-    if (!ck_pread(fd, s.hmem[0], n, off + done)) return ck_io_fail("rlm_load: cannot read", path);
-    CK(cudaMemcpyAsync((unsigned char*)r.dev + done, s.hmem[0], n, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    done += n;
-  }
-  return RLM_OK;
-}
-
-// Pack every table and write it from file offset *pos on; secs gets one section per table.  Chunk c packs into buffers
-// c & 1 on the handle's stream while the copy stream brings chunk c - 1 to the host and the host writes chunk c - 2.
-static int ck_tables_save(rlm_handle h, int fd, CkScratch& s, const std::vector<CkArr>& arrs, const std::vector<CkChunk>& ch,
-                          uint64_t* pos, std::vector<CkSection>& secs, const char* path) {
-  const long long M = h->cfg.memory_size, bmb = (M + 7) / 8;
-  const size_t C = ch.size();
-  CkSection cur = {};
-  std::vector<long long> cnt[2];
-  for (size_t c = 0; c <= C; ++c) {
-    const int b = (int)(c & 1);
-    if (c < C) {
-      const CkChunk& k = ch[c];
-      if (c >= 2) CK(cudaStreamWaitEvent(h->stream, s.ev_b[b], 0));  // (the copy of chunk c - 2 out of these buffers)
-      CK(rlm_launch_pack(s.d[b], arrs[k.arr].base + (size_t)k.t0 * M + k.lo, M, k.nt, k.len, h->stream));
-      CK(cudaMemcpyAsync(s.h_cnt[b], s.d[b].cnt, (size_t)k.nt * 8, cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaEventRecord(s.ev_a[b], h->stream));
-    }
-    if (c >= 1) {  // write chunk c - 1
-      const int pb = b ^ 1;
-      const CkChunk& k = ch[c - 1];
-      CK(cudaEventSynchronize(s.ev_b[pb]));
-      const long long bw = ck_bw(k.len);
-      long long v0 = 0;
-      for (int t = 0; t < k.nt; ++t) {
-        if (k.lo == 0) cur = {arrs[k.arr].id, (uint32_t)(k.t0 + t), *pos, 0, 0};
-        const long long n = cnt[pb][t];
-        if (!ck_pwrite(fd, s.h_bits[pb] + (size_t)t * bw, (size_t)((k.len + 7) / 8), cur.offset + k.lo / 8) ||
-            !ck_pwrite(fd, s.h_vals[pb] + v0, (size_t)n * 8, cur.offset + bmb + 8 * cur.count))
-          return ck_io_fail("rlm_save: cannot write", path);
-        v0 += n;
-        cur.count += n;
-        if (k.lo + k.len == M) {
-          cur.bytes = bmb + 8 * cur.count;
-          *pos = cur.offset + cur.bytes;
-          secs.push_back(cur);
-        }
-      }
-    }
-    if (c < C) {  // the counts of chunk c size its copy
-      const CkChunk& k = ch[c];
-      CK(cudaEventSynchronize(s.ev_a[b]));
-      cnt[b].assign(s.h_cnt[b], s.h_cnt[b] + k.nt);
-      long long tot = 0;
-      for (long long n : cnt[b]) tot += n;
-      CK(cudaStreamWaitEvent(s.cs, s.ev_a[b], 0));
-      CK(cudaMemcpyAsync(s.h_bits[b], s.d[b].bits, (size_t)(k.nt * ck_bw(k.len)) * 4, cudaMemcpyDeviceToHost, s.cs));
-      if (tot) CK(cudaMemcpyAsync(s.h_vals[b], s.d[b].vals, (size_t)tot * 8, cudaMemcpyDeviceToHost, s.cs));
-      CK(cudaEventRecord(s.ev_b[b], s.cs));
-    }
-  }
-  return RLM_OK;
-}
-
-// Read every table back.  pass 1 (count_only): only the bitmaps go to the device, and sub[c][t] gets the population of
-// chunk c's table t (the caller checks it against the stored counts).  pass 2: bitmaps and values, unpacked into the
-// arrays; the scan checks each table against sub and the unpack kernel writes nothing on a mismatch.  The host reads
-// chunk c + 1 while the copy stream uploads chunk c and the handle's stream unpacks it.
-static int ck_tables_load(rlm_handle h, int fd, CkScratch& s, const std::vector<CkArr>& arrs, const std::vector<CkChunk>& ch,
-                          const std::vector<const CkSection*>& sec_of, std::vector<std::vector<long long>>& sub, int count_only,
-                          const char* path) {
-  const long long M = h->cfg.memory_size, bmb = (M + 7) / 8;
-  const size_t C = ch.size();
-  std::vector<int> first(arrs.size() + 1, 0);  // section index of table 0 of each array
-  for (size_t a = 0; a < arrs.size(); ++a) first[a + 1] = first[a] + arrs[a].n;
-  std::vector<long long> run(sec_of.size(), 0);  // values read so far of each table (slices)
-  if (count_only) sub.assign(C, {});
-  for (size_t c = 0; c <= C; ++c) {
-    const int b = (int)(c & 1);
-    if (c < C) {
-      const CkChunk& k = ch[c];
-      if (c >= 2) CK(cudaEventSynchronize(s.ev_b[b]));  // chunk c - 2 is done with these buffers
-      const long long bw = ck_bw(k.len);
-      long long v0 = 0;
-      for (int t = 0; t < k.nt; ++t) {
-        const int si = first[k.arr] + k.t0 + t;
-        const CkSection& sc = *sec_of[si];
-        const size_t nb = (size_t)((k.len + 7) / 8);
-        unsigned char* bits = (unsigned char*)(s.h_bits[b] + (size_t)t * bw);
-        memset(bits + nb, 0, (size_t)bw * 4 - nb);
-        if (!ck_pread(fd, bits, nb, sc.offset + k.lo / 8)) return ck_io_fail("rlm_load: cannot read", path);
-        if (!count_only) {
-          const long long n = sub[c][t];
-          if (!ck_pread(fd, s.h_vals[b] + v0, (size_t)n * 8, sc.offset + bmb + 8 * run[si])) return ck_io_fail("rlm_load: cannot read", path);
-          s.h_expect[b][t] = n;
-          run[si] += n;
-          v0 += n;
-        }
-      }
-      CK(cudaMemcpyAsync(s.d[b].bits, s.h_bits[b], (size_t)(k.nt * bw) * 4, cudaMemcpyHostToDevice, s.cs));
-      if (!count_only) {
-        CK(cudaMemcpyAsync(s.d[b].expect, s.h_expect[b], (size_t)k.nt * 8, cudaMemcpyHostToDevice, s.cs));
-        if (v0) CK(cudaMemcpyAsync(s.d[b].vals, s.h_vals[b], (size_t)v0 * 8, cudaMemcpyHostToDevice, s.cs));
-      }
-      CK(cudaEventRecord(s.ev_a[b], s.cs));
-      CK(cudaStreamWaitEvent(h->stream, s.ev_a[b], 0));
-      CK(rlm_launch_unpack(s.d[b], arrs[k.arr].base + (size_t)k.t0 * M + k.lo, M, k.nt, k.len, count_only, h->stream));
-      if (count_only) CK(cudaMemcpyAsync(s.h_cnt[b], s.d[b].cnt, (size_t)k.nt * 8, cudaMemcpyDeviceToHost, h->stream));
-      CK(cudaEventRecord(s.ev_b[b], h->stream));
-    }
-    if (c >= 1 && count_only) {
-      CK(cudaEventSynchronize(s.ev_b[b ^ 1]));
-      sub[c - 1].assign(s.h_cnt[b ^ 1], s.h_cnt[b ^ 1] + ch[c - 1].nt);
-    }
-  }
-  CK(cudaStreamSynchronize(h->stream));
-  for (int b = 0; b < 2; ++b) CK(cudaMemcpy(s.h_err + b, s.d[b].err, sizeof(int), cudaMemcpyDeviceToHost));
-  return RLM_OK;
-}
-
-static int ck_library_fp(rlm_handle h, CkScratch& s, uint64_t* fp) {
-  const long long words = h->day_off.back() * (long long)sizeof(rlm_tick_msg) / 8;
-  CK(rlm_launch_fingerprint(h->ptr.tape, words, s.d_fp, h->n_sms, h->stream));
-  CK(cudaMemcpyAsync(fp, s.d_fp, 8, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return RLM_OK;
-}
-
-// the config with the fields a loading handle may differ in (and the struct's padding) cleared
-static rlm_config ck_norm(const rlm_config& in) {
-  rlm_config c = in;
-  c.device = 0;
-  memset(&c.flow, 0, sizeof(c.flow));
-  const size_t g1 = offsetof(rlm_config, lb_vwap) + sizeof(c.lb_vwap), g2 = offsetof(rlm_config, random_seed) + sizeof(c.random_seed);
-  memset((char*)&c + g1, 0, offsetof(rlm_config, pos_lb) - g1);
-  memset((char*)&c + g2, 0, offsetof(rlm_config, flow) - g2);
-  return c;
-}
-
-static const char* const k_ck_engine = "checkpoints need the tick-synchronous or round-paced engine (RLM_ENGINE=F|f|p run every step inside one launch)";
-
-int rlm_save(rlm_handle h, const char* path) {
-  API_LOCK;
-  if (!h || !path) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_save: null argument");
-  if (h->engine != 1) return fail(RLM_ERR_UNSUPPORTED, std::string("rlm_save: ") + k_ck_engine);
-  if (h->cfg.source == RLM_SOURCE_STREAM && h->stream_cursor < h->stream_ticks)
-    return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_save: " + std::to_string(h->stream_ticks - h->stream_cursor) +
-                                              " uploaded ticks are not consumed yet (run them, then save; upload the next ticks after rlm_load)");
-  int rc = tape_check(h);
-  if (rc) return rc;
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  rc = fix_records(h);
-  if (rc) return rc;
-  const CkView v = ck_view_of(h);
-  const std::vector<CkRaw> raw = ck_raw(h, v);
-  const std::vector<CkArr> arrs = ck_arrays(h);
-  const std::vector<CkChunk> ch = ck_chunks(arrs, h->cfg.memory_size);
-  int n_tables = 0;
-  for (const CkArr& a : arrs) n_tables += a.n;
-  CkScratch s;
-  rc = ck_scratch(h, s, ch);
-  if (rc) return rc;
-  CkHeader hd;
-  memset(&hd, 0, sizeof(hd));
-  memcpy(hd.magic, "RLMCKPT", 8);
-  hd.version = RLM_CK_VERSION;
-  hd.n_sections = (uint32_t)(raw.size() + n_tables);
-  hd.header_bytes = (uint32_t)(sizeof(CkHeader) + hd.n_sections * sizeof(CkSection));
-  hd.env_stride = (uint32_t)h->hp.env_stride;
-  hd.env_hdr_bytes = (uint32_t)sizeof(EnvHdr);
-  hd.model_log_cap = v.mlog_cap;
-  memcpy(&hd.cfg, &h->cfg, sizeof(rlm_config));
-  hd.alpha = h->alpha; hd.eps = h->eps; hd.tau = h->tau;
-  hd.launches = h->launches;
-  hd.run_seq = h->run_seq; hd.greedy = h->dyn.greedy; hd.backtest = h->dyn.backtest;
-  hd.n_days = v.n_days; hd.n_markets = v.n_markets; hd.has_env_market = v.has_env_market;
-  memcpy(&hd.shared_dyn, &h->shared_dyn, sizeof(DynParams));
-  if (h->cfg.source == RLM_SOURCE_TAPE) {
-    rc = ck_library_fp(h, s, &hd.library_fp);
-    if (rc) return rc;
-  }
-  const int fd = open(path, O_WRONLY | O_CREAT | O_TRUNC, 0644);
-  if (fd < 0) return fail(RLM_ERR_INVALID_ARGUMENT, std::string("rlm_save: cannot create ") + path + ": " + strerror(errno));
-  std::vector<CkSection> secs;
-  uint64_t pos = hd.header_bytes;
-  for (const CkRaw& r : raw) {
-    secs.push_back({r.id, 0, pos, r.bytes, 0});
-    rc = ck_raw_save(h, fd, s, r, pos, path);
-    if (rc) break;
-    pos += r.bytes;
-  }
-  if (!rc) rc = ck_tables_save(h, fd, s, arrs, ch, &pos, secs, path);
-  if (!rc) {
-    hd.file_bytes = pos;
-    if (!ck_pwrite(fd, &hd, sizeof(hd), 0) || !ck_pwrite(fd, secs.data(), secs.size() * sizeof(CkSection), sizeof(hd)))
-      rc = ck_io_fail("rlm_save: cannot write", path);
-  }
-  if (close(fd) != 0 && !rc) rc = ck_io_fail("rlm_save: cannot close", path);
-  if (rc) unlink(path);  // (no partial checkpoint is left behind)
-  return rc;
-}
-
-int rlm_load(rlm_handle h, const char* path) {
-  API_LOCK;
-  if (!h || !path) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_load: null argument");
-  if (h->engine != 1) return fail(RLM_ERR_UNSUPPORTED, std::string("rlm_load: ") + k_ck_engine);
-  const std::string P = std::string("rlm_load: ") + path + ": ";
-  const int fd = open(path, O_RDONLY);
-  if (fd < 0) return fail(RLM_ERR_INVALID_ARGUMENT, P + strerror(errno));
-  struct Closer { int fd; ~Closer() { close(fd); } } closer{fd};
-  struct stat st;
-  if (fstat(fd, &st) != 0) return fail(RLM_ERR_INVALID_ARGUMENT, P + strerror(errno));
-  const uint64_t size = (uint64_t)st.st_size;
-  // ---- everything is checked before anything of the handle changes
-  CkHeader hd;
-  if (size < sizeof(hd) || !ck_pread(fd, &hd, sizeof(hd), 0)) return fail(RLM_ERR_INVALID_ARGUMENT, P + "truncated header");
-  if (memcmp(hd.magic, "RLMCKPT", 8) != 0) return fail(RLM_ERR_INVALID_ARGUMENT, P + "not a checkpoint (bad magic)");
-  if (hd.version != RLM_CK_VERSION || hd.env_hdr_bytes != sizeof(EnvHdr))
-    return fail(RLM_ERR_INVALID_ARGUMENT, P + "layout version " + std::to_string(hd.version) + " / env header " + std::to_string(hd.env_hdr_bytes) +
-                                              " bytes; this library writes " + std::to_string(RLM_CK_VERSION) + " / " + std::to_string(sizeof(EnvHdr)));
-  if (hd.file_bytes != size) return fail(RLM_ERR_INVALID_ARGUMENT, P + "the file holds " + std::to_string(size) + " bytes, its header says " +
-                                                                       std::to_string(hd.file_bytes) + " (truncated?)");
-  {
-    const rlm_config a = ck_norm(hd.cfg), b = ck_norm(h->cfg);
-    if (memcmp(&a, &b, sizeof(a)) != 0 || hd.env_stride != (uint32_t)h->hp.env_stride)
-      return fail(RLM_ERR_INVALID_ARGUMENT, P + "the handle's config differs from the saved one (every field but device and flow must match)");
-  }
-  const bool tape = h->cfg.source == RLM_SOURCE_TAPE;
-  if (hd.model_log_cap < 0 || hd.model_log_cap > INT_MAX || hd.n_days < 0 || hd.n_markets < 0 || (hd.has_env_market & ~1) ||
-      (!tape && (hd.n_days || hd.n_markets || hd.has_env_market)))
-    return fail(RLM_ERR_INVALID_ARGUMENT, P + "corrupt header");
-  if (tape) {
-    int rc = tape_check(h);
-    if (rc) return rc;
-    if (hd.n_days != (int)h->day_off.size() - 1)
-      return fail(RLM_ERR_INVALID_ARGUMENT, P + "saved with a library of " + std::to_string(hd.n_days) + " days, the handle holds " +
-                                                std::to_string(h->day_off.size() - 1) + " (rlm_load_days the same library first)");
-  }
-  const int B = h->cfg.n_envs;
-  std::vector<int32_t> env_day(tape ? B : 0), day_market(hd.n_markets > 0 ? hd.n_days : 0), env_mkt(hd.has_env_market ? B : 0);
-  std::vector<int64_t> day_off(tape ? hd.n_days + 1 : 0);
-  CkView v = {};
-  v.mlog_cap = hd.model_log_cap; v.n_days = hd.n_days; v.n_markets = hd.n_markets; v.has_env_market = hd.has_env_market;
-  v.env_day = env_day.data(); v.day_off = day_off.data(); v.day_market = day_market.data(); v.env_mkt = env_mkt.data();
-  const std::vector<CkRaw> raw0 = ck_raw(h, v);
-  const std::vector<CkArr> arrs = ck_arrays(h);
-  const std::vector<CkChunk> ch = ck_chunks(arrs, h->cfg.memory_size);
-  const long long M = h->cfg.memory_size, bmb = (M + 7) / 8;
-  size_t n_tables = 0;
-  for (const CkArr& a : arrs) n_tables += a.n;
-  if (hd.n_sections != raw0.size() + n_tables || hd.header_bytes != sizeof(CkHeader) + hd.n_sections * sizeof(CkSection))
-    return fail(RLM_ERR_INVALID_ARGUMENT, P + "the section table does not fit the handle's config");
-  std::vector<CkSection> secs(hd.n_sections);
-  if (!ck_pread(fd, secs.data(), secs.size() * sizeof(CkSection), sizeof(hd))) return fail(RLM_ERR_INVALID_ARGUMENT, P + "truncated section table");
-  {
-    uint64_t pos = hd.header_bytes;
-    size_t i = 0;
-    for (const CkRaw& r : raw0) {
-      const CkSection& sc = secs[i++];
-      if (sc.id != r.id || sc.offset != pos || sc.bytes != r.bytes) return fail(RLM_ERR_INVALID_ARGUMENT, P + "section " + std::to_string(i - 1) + " does not fit the handle");
-      pos += sc.bytes;
-    }
-    for (const CkArr& a : arrs)
-      for (int t = 0; t < a.n; ++t) {
-        const CkSection& sc = secs[i++];
-        if (sc.id != a.id || sc.table != (uint32_t)t || sc.offset != pos || sc.count > (uint64_t)M || sc.bytes != (uint64_t)bmb + 8 * sc.count)
-          return fail(RLM_ERR_INVALID_ARGUMENT, P + "packed table section " + std::to_string(i - 1) + " is malformed");
-        pos += sc.bytes;
-      }
-    if (pos != size) return fail(RLM_ERR_INVALID_ARGUMENT, P + "the sections do not add up to the file's length");
-  }
-  for (size_t i = 0; i < raw0.size(); ++i)  // host sections: small, read now and checked
-    if (raw0[i].host && !ck_pread(fd, raw0[i].host, raw0[i].bytes, secs[i].offset)) return fail(RLM_ERR_INVALID_ARGUMENT, P + "cannot read");
-  if (tape) {
-    if (day_off != h->day_off) return fail(RLM_ERR_INVALID_ARGUMENT, P + "the handle's day library has other day offsets than the saved one");
-    for (int32_t d : env_day) if (d < 0 || d >= hd.n_days) return fail(RLM_ERR_INVALID_ARGUMENT, P + "corrupt day assignment");
-    for (int32_t k : day_market) if (k < 0 || k >= hd.n_markets) return fail(RLM_ERR_INVALID_ARGUMENT, P + "corrupt day markets");
-    for (int32_t k : env_mkt) if (k < -1 || k >= hd.n_markets) return fail(RLM_ERR_INVALID_ARGUMENT, P + "corrupt env markets");
-  }
-  CK(cudaSetDevice(h->cfg.device));
-  CK(cudaStreamSynchronize(h->stream));
-  CkScratch s;
-  int rc = ck_scratch(h, s, ch);
-  if (rc) return rc;
-  if (tape) {
-    uint64_t fp = 0;
-    rc = ck_library_fp(h, s, &fp);
-    if (rc) return rc;
-    if (fp != hd.library_fp) return fail(RLM_ERR_INVALID_ARGUMENT, P + "the handle's day library differs from the saved one (fingerprint)");
-  }
-  std::vector<const CkSection*> sec_of;
-  for (size_t i = raw0.size(); i < secs.size(); ++i) sec_of.push_back(&secs[i]);
-  std::vector<std::vector<long long>> sub;
-  rc = ck_tables_load(h, fd, s, arrs, ch, sec_of, sub, 1, path);
-  if (rc) return rc;
-  {
-    std::vector<long long> tot(sec_of.size(), 0);
-    std::vector<int> first(arrs.size() + 1, 0);
-    for (size_t a = 0; a < arrs.size(); ++a) first[a + 1] = first[a] + arrs[a].n;
-    for (size_t c = 0; c < ch.size(); ++c)
-      for (int t = 0; t < ch[c].nt; ++t) tot[first[ch[c].arr] + ch[c].t0 + t] += sub[c][t];
-    bool bad = s.h_err[0] || s.h_err[1];
-    for (size_t i = 0; i < tot.size(); ++i) bad = bad || tot[i] != (long long)sec_of[i]->count;
-    if (bad) return fail(RLM_ERR_INVALID_ARGUMENT, P + "corrupt packed table (bitmap population differs from the stored value count)");
-  }
-  // ---- the new buffers, before anything is replaced
-  ModelLogPtrs L = {};
-  VenueD* d_markets = nullptr;
-  int *d_env_market = nullptr, *d_rec_fixed = nullptr;
-  {
-    cudaError_t ce = cudaSuccess;
-    if (hd.model_log_cap > 0) {
-      L.cap = hd.model_log_cap;
-      ce = cudaMalloc(&L.acc, (size_t)B * sizeof(ModelLogAcc));
-      if (ce == cudaSuccess) ce = cudaMalloc(&L.written, (size_t)B * 8);
-      if (ce == cudaSuccess) ce = cudaMalloc(&L.rows, (size_t)B * (size_t)L.cap * 8);
-    }
-    if (ce == cudaSuccess && hd.n_markets > 0) ce = cudaMalloc(&d_markets, (size_t)hd.n_markets * sizeof(VenueD));
-    if (ce == cudaSuccess && hd.has_env_market && !h->dm.env_market) {
-      ce = cudaMalloc(&d_env_market, (size_t)B * sizeof(int));
-      if (ce == cudaSuccess && h->hp.record_envs > 0) ce = cudaMalloc(&d_rec_fixed, (size_t)h->hp.record_envs * sizeof(int));
-    }
-    if (ce != cudaSuccess) {
-      cudaFree(L.acc); cudaFree(L.written); cudaFree(L.rows); cudaFree(d_markets); cudaFree(d_env_market); cudaFree(d_rec_fixed);
-      CK(ce);
-    }
-  }
-  // ---- commit
-  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
-  h->graphs.clear();
-  h->graph_warm = false;
-  cudaFree(h->mlog.acc); cudaFree(h->mlog.written); cudaFree(h->mlog.rows);
-  h->mlog = L;
-  cudaFree((void*)h->dm.markets);
-  h->dm.markets = d_markets;
-  h->n_markets = hd.n_markets;
-  if (!hd.has_env_market) {
-    cudaFree(h->dm.env_market); cudaFree(h->dm.rec_fixed);
-    h->dm.env_market = nullptr; h->dm.rec_fixed = nullptr;
-  } else if (d_env_market) {
-    h->dm.env_market = d_env_market; h->dm.rec_fixed = d_rec_fixed;
-  }
-  h->env_day = env_day; h->day_market = day_market; h->env_mkt = env_mkt;
-  v = ck_view_of(h);
-  const std::vector<CkRaw> raw = ck_raw(h, v);
-  for (size_t i = 0; i < raw.size() && !rc; ++i)
-    if (raw[i].dev) rc = ck_raw_load(h, fd, s, raw[i], secs[i].offset, path);
-  if (!rc && hd.has_env_market) {
-    CK(cudaMemcpy(h->dm.env_market, h->env_mkt.data(), (size_t)B * sizeof(int), cudaMemcpyHostToDevice));
-  }
-  if (!rc) rc = ck_tables_load(h, fd, s, arrs, ch, sec_of, sub, 0, path);
-  if (!rc && (s.h_err[0] || s.h_err[1])) rc = fail(RLM_ERR_RUNTIME, P + "the file changed while it was loaded; the handle's state is undefined");
-  if (rc) return rc;
-  h->alpha = hd.alpha; h->eps = hd.eps; h->tau = hd.tau;
-  h->launches = hd.launches;
-  h->run_seq = hd.run_seq;
-  h->dyn.greedy = hd.greedy; h->dyn.backtest = hd.backtest;
-  memcpy(&h->shared_dyn, &hd.shared_dyn, sizeof(DynParams));
-  memcpy(&h->cfg.flow, &hd.cfg.flow, sizeof(rlm_flow_params));
-  h->hp.flow = h->cfg.flow;
-  h->rec_dirty = false;
-  h->stream_ticks = 0; h->stream_cursor = 0;
-  day_markets_on(h, h->dm.markets != nullptr);  // (and the parameters are uploaded again before the next launch)
   return RLM_OK;
 }
 
@@ -2346,61 +1621,48 @@ static int test_setup(const rlm_config* cfg, rlm_handle_s& tmp) {
   return RLM_OK;
 }
 
+// device memory of one unit-level call, freed on every path
+struct DevBuf {
+  void* p = nullptr;
+  ~DevBuf() { cudaFree(p); }
+};
+// One unit-level kernel run: the constants of cfg uploaded (unless null), in_bytes from `in` to the device,
+// launch(d_in, d_out), out_bytes of d_out back to `out`.
+template <class Launch>
+static int test_run(const rlm_config* cfg, const void* in, size_t in_bytes, void* out, size_t out_bytes, Launch launch) {
+  if (cfg) {
+    rlm_handle_s tmp;
+    const int rc = test_setup(cfg, tmp);
+    if (rc) return rc;
+  }
+  DevBuf d_in, d_out;
+  CK(cudaMalloc(&d_in.p, in_bytes)); CK(cudaMalloc(&d_out.p, out_bytes));
+  CK(cudaMemcpy(d_in.p, in, in_bytes, cudaMemcpyHostToDevice));
+  CK(launch(d_in.p, d_out.p));
+  CK(cudaMemcpy(out, d_out.p, out_bytes, cudaMemcpyDeviceToHost));
+  return RLM_OK;
+}
+
 int rlm_test_to_ticks(const rlm_config* cfg, const double* px, int32_t n, int32_t* out) {
   API_LOCK;
-  rlm_handle_s tmp;
-  int rc = test_setup(cfg, tmp);
-  if (rc) return rc;
-  double* d_in; int* d_out;
-  CK(cudaMalloc(&d_in, n * 8)); CK(cudaMalloc(&d_out, n * 4));
-  CK(cudaMemcpy(d_in, px, n * 8, cudaMemcpyHostToDevice));
-  CK(rlm_launch_test_to_ticks(d_in, n, d_out));
-  CK(cudaMemcpy(out, d_out, n * 4, cudaMemcpyDeviceToHost));
-  cudaFree(d_in); cudaFree(d_out);
-  return RLM_OK;
+  return test_run(cfg, px, n * 8, out, n * 4, [&](void* in, void* o) { return rlm_launch_test_to_ticks((const double*)in, n, (int*)o); });
 }
 int rlm_test_to_price(const rlm_config* cfg, const int32_t* ticks, int32_t n, double* out) {
   API_LOCK;
-  rlm_handle_s tmp;
-  int rc = test_setup(cfg, tmp);
-  if (rc) return rc;
-  int* d_in; double* d_out;
-  CK(cudaMalloc(&d_in, n * 4)); CK(cudaMalloc(&d_out, n * 8));
-  CK(cudaMemcpy(d_in, ticks, n * 4, cudaMemcpyHostToDevice));
-  CK(rlm_launch_test_to_price(d_in, n, d_out));
-  CK(cudaMemcpy(out, d_out, n * 8, cudaMemcpyDeviceToHost));
-  cudaFree(d_in); cudaFree(d_out);
-  return RLM_OK;
+  return test_run(cfg, ticks, n * 4, out, n * 8, [&](void* in, void* o) { return rlm_launch_test_to_price((const int*)in, n, (double*)o); });
 }
 int rlm_test_tiles(const rlm_config* cfg, const float* vars, int32_t n, int32_t* out) {
   API_LOCK;
-  rlm_handle_s tmp;
-  int rc = test_setup(cfg, tmp);
-  if (rc) return rc;
-  float* d_in; int* d_out;
   size_t nin = (size_t)n * cfg->n_state_vars, nout = (size_t)n * cfg->n_actions * 96;
-  CK(cudaMalloc(&d_in, nin * 4)); CK(cudaMalloc(&d_out, nout * 4));
-  CK(cudaMemcpy(d_in, vars, nin * 4, cudaMemcpyHostToDevice));
-  CK(rlm_launch_test_tiles(d_in, n, d_out));
-  CK(cudaMemcpy(out, d_out, nout * 4, cudaMemcpyDeviceToHost));
-  cudaFree(d_in); cudaFree(d_out);
-  return RLM_OK;
+  return test_run(cfg, vars, nin * 4, out, nout * 4, [&](void* in, void* o) { return rlm_launch_test_tiles((const float*)in, n, (int*)o); });
 }
 int rlm_test_learner_tiles(const rlm_config* cfg, int32_t form, const float* vars, int32_t n, int32_t* out) {
   API_LOCK;
   if (form < RLM_TILES_THREE_WARP || form > RLM_TILES_TRACE_GROUP0) return fail(RLM_ERR_INVALID_ARGUMENT, "unknown tile form");
   if (form == RLM_TILES_STAGED && cfg->memory_size > 8192) return fail(RLM_ERR_UNSUPPORTED, "the staged learner holds tables of at most 8192 weights");
-  rlm_handle_s tmp;
-  int rc = test_setup(cfg, tmp);
-  if (rc) return rc;
-  float* d_in; int* d_out;
   size_t nin = (size_t)n * cfg->n_state_vars, nout = (size_t)n * cfg->n_actions * (form == RLM_TILES_TRACE_GROUP0 ? 32 : 96);
-  CK(cudaMalloc(&d_in, nin * 4)); CK(cudaMalloc(&d_out, nout * 4));
-  CK(cudaMemcpy(d_in, vars, nin * 4, cudaMemcpyHostToDevice));
-  CK(rlm_launch_test_learner_tiles(form, d_in, n, d_out));
-  CK(cudaMemcpy(out, d_out, nout * 4, cudaMemcpyDeviceToHost));
-  cudaFree(d_in); cudaFree(d_out);
-  return RLM_OK;
+  return test_run(cfg, vars, nin * 4, out, nout * 4,
+                  [&](void* in, void* o) { return rlm_launch_test_learner_tiles(form, (const float*)in, n, (int*)o); });
 }
 int rlm_test_order(int64_t size, int64_t q_head, const rlm_order_op* ops, int32_t n_ops, rlm_order_state* out) {
   API_LOCK;
@@ -2411,13 +1673,9 @@ int rlm_test_order(int64_t size, int64_t q_head, const rlm_order_op* ops, int32_
   for (int i = 0; i < n_ops; ++i)
     if ((ops[i].op == 0 || ops[i].op == 1) && ops[i].arg < 0)
       return fail(RLM_ERR_RUNTIME, ops[i].op == 0 ? "Transaction volume must be positive." : "Cancellation volume must be positive.");  // order.cpp:56-57,86-87
-  rlm_order_op* d_ops; rlm_order_state* d_out;
-  CK(cudaMalloc(&d_ops, n_ops * sizeof(rlm_order_op))); CK(cudaMalloc(&d_out, n_ops * sizeof(rlm_order_state)));
-  CK(cudaMemcpy(d_ops, ops, n_ops * sizeof(rlm_order_op), cudaMemcpyHostToDevice));
-  CK(rlm_launch_test_order(size, q_head, d_ops, n_ops, d_out));
-  CK(cudaMemcpy(out, d_out, n_ops * sizeof(rlm_order_state), cudaMemcpyDeviceToHost));
-  cudaFree(d_ops); cudaFree(d_out);
-  return RLM_OK;
+  return test_run(nullptr, ops, n_ops * sizeof(rlm_order_op), out, n_ops * sizeof(rlm_order_state), [&](void* in, void* o) {
+    return rlm_launch_test_order(size, q_head, (const rlm_order_op*)in, n_ops, (rlm_order_state*)o);
+  });
 }
 int rlm_test_rolling_mean(int32_t window, const double* vals, int32_t n, double* out) {
   API_LOCK;
@@ -2428,14 +1686,10 @@ int rlm_test_rolling_mean(int32_t window, const double* vals, int32_t n, double*
   rlm_handle_s tmp;
   int rc = test_setup(&cfg, tmp);
   if (rc) return rc;
-  double *d_in, *d_out, *d_ring; EnvHdr* d_e;
-  CK(cudaMalloc(&d_in, n * 8)); CK(cudaMalloc(&d_out, n * 16)); CK(cudaMalloc(&d_ring, (size_t)tmp.hp.ring_total * 8)); CK(cudaMalloc(&d_e, sizeof(EnvHdr)));
-  CK(cudaMemset(d_ring, 0, (size_t)tmp.hp.ring_total * 8)); CK(cudaMemset(d_e, 0, sizeof(EnvHdr)));
-  CK(cudaMemcpy(d_in, vals, n * 8, cudaMemcpyHostToDevice));
-  CK(rlm_launch_test_rolling_mean(d_in, n, d_out, d_ring, d_e));
-  CK(cudaMemcpy(out, d_out, n * 16, cudaMemcpyDeviceToHost));
-  cudaFree(d_in); cudaFree(d_out); cudaFree(d_ring); cudaFree(d_e);
-  return RLM_OK;
+  DevBuf d_ring, d_e;
+  CK(cudaMalloc(&d_ring.p, (size_t)tmp.hp.ring_total * 8)); CK(cudaMalloc(&d_e.p, sizeof(EnvHdr)));
+  CK(cudaMemset(d_ring.p, 0, (size_t)tmp.hp.ring_total * 8)); CK(cudaMemset(d_e.p, 0, sizeof(EnvHdr)));
+  return test_run(nullptr, vals, n * 8, out, n * 16, [&](void* in, void* o) {
+    return rlm_launch_test_rolling_mean((const double*)in, n, (double*)o, (double*)d_ring.p, (EnvHdr*)d_e.p);
+  });
 }
-
-}  // extern "C"

@@ -69,14 +69,14 @@ double pkey(double p) { return rint(p * 10000.0); }
 }  // namespace
 
 extern "C" const char* rlm_last_error(void);
-int rlm_set_error_(int code, const std::string& msg);  // rlm_api.cu
+int fail(int code, const std::string& msg);  // rlm_handle.h
 
 extern "C" int rlm_ingest_csv(const char* md_path, const char* tas_path, rlm_tick_msg* out, int64_t cap, int64_t* n_msgs, int64_t* n_ticks) {
-  if (!md_path || !tas_path || !n_msgs) return rlm_set_error_(RLM_ERR_INVALID_ARGUMENT, "rlm_ingest_csv: null argument");
+  if (!md_path || !tas_path || !n_msgs) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_ingest_csv: null argument");
   std::string err;
   std::vector<std::string> lines, cols;
   std::vector<MdRow> rows;
-  if (!read_lines(md_path, lines, err)) return rlm_set_error_(RLM_ERR_INVALID_ARGUMENT, err);
+  if (!read_lines(md_path, lines, err)) return fail(RLM_ERR_INVALID_ARGUMENT, err);
   std::vector<std::string> piece;
   cols.clear();
   for (const std::string& ln : lines) {
@@ -102,7 +102,7 @@ extern "C" int rlm_ingest_csv(const char* md_path, const char* tas_path, rlm_tic
   }
   lines.clear();
   std::vector<Print> prints;
-  if (!read_lines(tas_path, lines, err)) return rlm_set_error_(RLM_ERR_INVALID_ARGUMENT, err);
+  if (!read_lines(tas_path, lines, err)) return fail(RLM_ERR_INVALID_ARGUMENT, err);
   cols.clear();
   for (const std::string& ln : lines) {
     split(ln, piece);  // TimeAndSales::_LoadRow (basic.cpp:136-148): same buffer behaviour, 4 columns
@@ -120,7 +120,7 @@ extern "C" int rlm_ingest_csv(const char* md_path, const char* tas_path, rlm_tic
   for (size_t i = 0; i < rows.size(); ++i)
     for (int l = 1; l < 5; ++l)
       if (!(pkey(rows[i].ap[l]) > pkey(rows[i].ap[l - 1])) || !(pkey(rows[i].bp[l]) < pkey(rows[i].bp[l - 1])))
-        return rlm_set_error_(RLM_ERR_UNSUPPORTED, "rlm_ingest_csv: depth row " + std::to_string(i) + " is not strictly ordered best-first (AP ascending, BP descending)");
+        return fail(RLM_ERR_UNSUPPORTED, "rlm_ingest_csv: depth row " + std::to_string(i) + " is not strictly ordered best-first (AP ascending, BP descending)");
 
   int64_t n_out = 0, ticks = 0;
   auto emit = [&](const rlm_tick_msg& m) { if (out && n_out < cap) out[n_out] = m; ++n_out; };
@@ -141,7 +141,7 @@ extern "C" int rlm_ingest_csv(const char* md_path, const char* tas_path, rlm_tic
       ++j;
     }
     if (agg.size() > RLM_TX_CAP)
-      return rlm_set_error_(RLM_ERR_UNSUPPORTED, "rlm_ingest_csv: more than " + std::to_string(RLM_TX_CAP) + " distinct print prices in the tick of depth row " + std::to_string(i));
+      return fail(RLM_ERR_UNSUPPORTED, "rlm_ingest_csv: more than " + std::to_string(RLM_TX_CAP) + " distinct print prices in the tick of depth row " + std::to_string(i));
     // all but the last RLM_N_TX_MAX prices travel ahead in RLM_TICK_TX_MORE messages
     size_t lead = agg.size() > RLM_N_TX_MAX ? agg.size() - RLM_N_TX_MAX : 0, a = 0;
     while (a < lead) {
@@ -188,6 +188,6 @@ extern "C" int rlm_ingest_csv(const char* md_path, const char* tas_path, rlm_tic
   }
   *n_msgs = n_out;
   if (n_ticks) *n_ticks = ticks;
-  if (out && n_out > cap) return rlm_set_error_(RLM_ERR_INVALID_ARGUMENT, "rlm_ingest_csv: output buffer too small");
+  if (out && n_out > cap) return fail(RLM_ERR_INVALID_ARGUMENT, "rlm_ingest_csv: output buffer too small");
   return RLM_OK;
 }

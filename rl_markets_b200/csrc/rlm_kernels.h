@@ -37,20 +37,6 @@ cudaError_t rlm_launch_env_market(const DevPtrs& ptr, int env0, int n, const int
 cudaError_t rlm_launch_fix_terminal(const DevPtrs& ptr, int record_envs, cudaStream_t st);
 cudaError_t rlm_launch_model_log(const ModelLogPtrs& L, const DevPtrs& ptr, int env_stride, int env0, int n, cudaStream_t st);
 cudaError_t rlm_launch_model_log_baseline(const ModelLogPtrs& L, const DevPtrs& ptr, int env_stride, int n_envs, cudaStream_t st);
-// checkpoints (rlm_checkpoint.cu): device scratch of one chunk of packed tables
-#define RLM_CK_TILE 8192  // words per block of the pack / unpack kernels
-struct CkChunkDev {
-  double* vals;       // the chunk's nonzero words, table after table
-  unsigned* bits;     // [nt][ceil(len / 32)] bitmap words
-  int* blk_cnt;       // [nt * bpt] population of each block's tile
-  long long* off;     // [nt * bpt + 1] exclusive offsets of the tiles' values
-  long long* cnt;     // [nt] values of each table
-  long long* expect;  // [nt] unpack: the stored value count of each table
-  int* err;           // unpack: nonzero = the bitmap does not match the stored counts
-};
-cudaError_t rlm_launch_pack(const CkChunkDev& c, const double* src, long long tstride, int nt, long long len, cudaStream_t st);
-cudaError_t rlm_launch_unpack(const CkChunkDev& c, double* dst, long long tstride, int nt, long long len, int count_only, cudaStream_t st);
-cudaError_t rlm_launch_fingerprint(const void* data, long long n_words, unsigned long long* out, int n_sms, cudaStream_t st);
 cudaError_t rlm_launch_test_to_ticks(const double* px, int n, int* out);
 cudaError_t rlm_launch_test_to_price(const int* t, int n, double* out);
 cudaError_t rlm_launch_test_tiles(const float* vars, int n, int* out);
