@@ -1594,6 +1594,14 @@ int rlm_get_kernel_times(rlm_handle h, double* env_ms, double* agent_ms, int64_t
   if (agent_launches) *agent_launches = h->prof_agent_launches;
   return RLM_OK;
 }
+#ifdef RLM_TIMING
+// the what-if switches of RLM_DEBUG_FLAGS on a live handle, so that one trained state can be timed under each of them
+extern "C" int rlm_debug_set_flags(rlm_handle h, int32_t flags) {
+  if (!h) return fail(RLM_ERR_INVALID_ARGUMENT, "null handle");
+  h->dyn.debug_flags = flags;
+  return RLM_OK;
+}
+#endif
 
 int rlm_flow_generate(const rlm_flow_params* p, int64_t env_index, int64_t first_tick, int32_t n_ticks, rlm_tick_msg* out) {
   if (!p || !out || n_ticks < 0 || first_tick < 0) return fail(RLM_ERR_INVALID_ARGUMENT, "bad arguments");

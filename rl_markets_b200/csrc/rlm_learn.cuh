@@ -101,43 +101,47 @@ __device__ __forceinline__ void ut_insert(int* ut, int f, float ev) {  // every 
   while (atomicCAS(&ut[slot], HS_EMPTY, f) != HS_EMPTY) slot = (slot + 1) & (UT_SLOTS - 1);
   ((float*)(ut + UT_SLOTS))[slot] = ev;
 }
-// the step's tile indices are re-derived from the hash sums (two instructions each for a power-of-two M): no index table
-__device__ __forceinline__ void ln_patch_local(const int* ut, double scaled_update, unsigned long long s0, unsigned long long s1, unsigned long long s2,
-                                               bool null_state, int lane, double* V) {
+// the step's tile indices are re-derived from the hash sums (two instructions each for a power-of-two M): no index table.
+// The table holds a few dozen of its 1024 slots (Z + 32 at most), so nearly every tile's first probe finds an empty slot:
+// the first probes of all 27 tiles go first, and only the few tiles whose first slot is taken (the update landed on them,
+// or another feature's probe chain passes by) walk the table.  Returns: this lane patched a weight.
+template <bool POW2>
+__device__ __forceinline__ unsigned ln_patch_candidates(const int* ut, const LnSums& h) {
   const int A = P.n_actions;
+  unsigned cand = 0;
+#pragma unroll
+  for (int k = 0; k < 3 * RLM_MAX_ACTIONS; ++k)
+    if ((k % RLM_MAX_ACTIONS) < A && ut[ut_hash(ln_tile<POW2>(h, k))] != HS_EMPTY) cand |= 1u << k;
+  return cand;
+}
+__device__ __forceinline__ bool ln_patch_local(const int* ut, double scaled_update, unsigned long long s0, unsigned long long s1, unsigned long long s2,
+                                               bool null_state, int lane, double* V) {
   const float* uv = (const float*)(ut + UT_SLOTS);
-  const bool pow2 = P.m_pow2 != 0;
-  const unsigned mask = (unsigned)(P.memory_size - 1);
-  // rolled over the actions (this runs once per step: code size is time), the three feature groups of one action side by
-  // side: three independent index -> hash -> key chains per iteration instead of one
-#pragma unroll 1
-  for (int a = 0; a < A; ++a) {
-    int f[3], key[3];
-    unsigned slot[3];
-#pragma unroll
-    for (int g = 0; g < 3; ++g) {
-      const unsigned r = P.rg[g][a];
-      const unsigned long long sg = g == 0 ? s0 : (g == 1 ? s1 : s2);
-      f[g] = null_state ? 0 : (pow2 ? (int)(((unsigned)sg + r) & mask) : mod_m(sg + r));
-    }
-#pragma unroll
-    for (int g = 0; g < 3; ++g) { slot[g] = ut_hash(f[g]); key[g] = ut[slot[g]]; }
-#pragma unroll
-    for (int g = 0; g < 3; ++g) {
-      while (key[g] != HS_EMPTY && key[g] != f[g]) { slot[g] = (slot[g] + 1) & (UT_SLOTS - 1); key[g] = ut[slot[g]]; }
-      if (key[g] == f[g]) {
-        const int at = a * LN_VROW + g * 32 + lane;
-        V[at] = V[at] + scaled_update * (double)uv[slot[g]];
-      }
+  LnSums h;
+  h.s[0] = s0; h.s[1] = s1; h.s[2] = s2; h.null_state = null_state;
+  unsigned cand = P.m_pow2 ? ln_patch_candidates<true>(ut, h) : ln_patch_candidates<false>(ut, h);
+  bool patched = false;
+  while (cand) {
+    const int k = __ffs(cand) - 1;
+    cand &= cand - 1;
+    const int f = P.m_pow2 ? ln_tile<true>(h, k) : ln_tile<false>(h, k);
+    unsigned slot = ut_hash(f);
+    int key = ut[slot];
+    while (key != HS_EMPTY && key != f) { slot = (slot + 1) & (UT_SLOTS - 1); key = ut[slot]; }
+    if (key == f) {
+      const int at = (k % RLM_MAX_ACTIONS) * LN_VROW + (k / RLM_MAX_ACTIONS) * 32 + lane;
+      V[at] = V[at] + scaled_update * (double)uv[slot];
+      patched = true;
     }
   }
+  return patched;
 }
 
 // (the rare mid-list drain of a full table calls this copy; the step's final batch is patched inline)
-__device__ __noinline__ void ln_patch_local_ool(const int* ut, double scaled_update, unsigned long long s0, unsigned long long s1, unsigned long long s2,
+__device__ __noinline__ bool ln_patch_local_ool(const int* ut, double scaled_update, unsigned long long s0, unsigned long long s1, unsigned long long s2,
                                                 bool null_state, int lane, double* V) {
   ASSUME_SHARED(ut); ASSUME_SHARED(V);
-  ln_patch_local(ut, scaled_update, s0, s1, s2, null_state, lane, V);
+  return ln_patch_local(ut, scaled_update, s0, s1, s2, null_state, lane, V);
 }
 
 // ---- exact-order sum of agent.cpp:117-135 over one action row of raw weights: 16 blocks of 8; block b+1 is loaded
@@ -243,14 +247,15 @@ __device__ __forceinline__ void ln_tt_build(int* tt, const AgentD& ag, int lane)
 // track: `ut` (cleared by the caller) takes the surviving entries, UT_MAX_ENTRIES at a time: when the table is full its
 // updates are added to the weights of the to-state right away (ln_patch_local on Vp; every feature is in the list once,
 // so every weight still gets at most one addition) and the table starts over.  The caller patches the last batch.
+// patched |= a mid-list drain added an update to a weight of Vp.
 __device__ __forceinline__ int ln_trace_pass(AgentD& e, const int* tt, int* ut, bool track, int* tf, float* te, double* theta, int action,
-                                          float rate, double scaled_update, int lane, const LnSums& h, double* Vp) {
+                                          float rate, double scaled_update, int lane, const LnSums& h, double* Vp, bool& patched) {
   const bool null_from = e.null_from != 0;
   const int b0 = e.from_base0[lane];
   const float tol = 0.01f;
   int w = 0;
   int ins = 0;  // entries in `ut` (warp-uniform)
-#define LN_UT_FLUSH() do { __syncwarp(); ln_patch_local_ool(ut, scaled_update, h.s[0], h.s[1], h.s[2], h.null_state, lane, Vp); __syncwarp(); ut_clear(ut, lane); __syncwarp(); ins = 0; } while (0)
+#define LN_UT_FLUSH() do { __syncwarp(); patched |= ln_patch_local_ool(ut, scaled_update, h.s[0], h.s[1], h.s[2], h.null_state, lane, Vp); __syncwarp(); ut_clear(ut, lane); __syncwarp(); ins = 0; } while (0)
   if (rate != 0.0f) {
     const int n = e.n_traces;
 #pragma unroll 1
@@ -263,14 +268,33 @@ __device__ __forceinline__ int ln_trace_pass(AgentD& e, const int* tt, int* ut, 
         fq[k] = (i < n) ? __ldcg(tf + i) : 0;
         eq[k] = (i < n) ? __ldcg(te + i) : 0.0f;
       }
+      // the keep decisions of the whole batch first: their tile-table probes are independent, so all first probes are in
+      // flight together, and no store or table insert of one entry waits for the probes of the next
+      bool kq[TR_AHEAD];
+      unsigned slot[TR_AHEAD];
+      int key[TR_AHEAD];
+#pragma unroll
+      for (int k = 0; k < TR_AHEAD; ++k) {
+        kq[k] = (base + 32 * k + lane < n) && !(eq[k] * rate < tol);
+        slot[k] = tt_hash(fq[k]);
+        key[k] = (kq[k] && !null_from) ? tt[slot[k]] : HS_EMPTY;
+      }
+#pragma unroll
+      for (int k = 0; k < TR_AHEAD; ++k) {
+        if (null_from) {
+          kq[k] = kq[k] && fq[k] != 0;  // (the null State's one feature 0 is last written by action A-1)
+        } else if (kq[k]) {  // ptt_last_writer(tt, f) < 0
+          while (key[k] != HS_EMPTY && (key[k] >> 4) != fq[k]) { slot[k] = (slot[k] + 1) & (TT_SLOTS - 1); key[k] = tt[slot[k]]; }
+          kq[k] = key[k] == HS_EMPTY;
+        }
+      }
 #pragma unroll
       for (int k = 0; k < TR_AHEAD; ++k) {
         if (base + 32 * k < n) {  // warp-uniform
           const int i = base + 32 * k + lane;
           const int f = fq[k];
           const float ev = eq[k] * rate;
-          bool keep = (i < n) && !(ev < tol);
-          if (keep) keep = (null_from ? (f == 0 ? P.n_actions - 1 : -1) : ptt_last_writer(tt, f)) < 0;
+          const bool keep = kq[k];
           const unsigned mask = __ballot_sync(FULL, keep);
           const int pos = w + __popc(mask & ((1u << lane) - 1u));
           if (track && ins + __popc(mask) > UT_MAX_ENTRIES) LN_UT_FLUSH();
@@ -471,7 +495,10 @@ __device__ __forceinline__ void ln_step(const DevPtrs& ptr, const DynParams& D, 
       ln_td_qlearn(ag, qpre, q_pre_a, D, lane, rate, scaled);
     } else {
       if (lane == 0)
-        td_decision(ag, q_pre_a, q_pre_b, ptr.mt_pol + (size_t)env * 312, ptr.mt_agt ? ptr.mt_agt + (size_t)env * 312 : nullptr, D, dec);
+        {  // (by a copy: a reference to the kernel parameter itself would put all of it in local memory for the whole step)
+          const DynParams dc = D;
+          td_decision(ag, q_pre_a, q_pre_b, ptr.mt_pol + (size_t)env * 312, ptr.mt_agt ? ptr.mt_agt + (size_t)env * 312 : nullptr, dc, dec);
+        }
       __syncwarp();
       rate = (float)dec[0];
       scaled = dec[1];
@@ -485,8 +512,9 @@ __device__ __forceinline__ void ln_step(const DevPtrs& ptr, const DynParams& D, 
     if (stage == 1) th = table ? ptr.dtheta + P.memory_size : ptr.dtheta;  // accumulate, apply after the all-reduce
     const bool local_patch = (stage == 0) && !dbg_nopatch;
     if (local_patch) { ut_clear(ut, lane); __syncwarp(); }
+    bool patched = false;
     const int nz = ln_trace_pass(ag, tt, ut, local_patch, tf, te, th, ag.cur_action, rate, scaled, lane, h,
-                                 V + (table ? RLM_MAX_ACTIONS * LN_VROW : 0));
+                                 V + (table ? RLM_MAX_ACTIONS * LN_VROW : 0), patched);
     if (lane == 0) { ag.n_traces = nz; ag.sum_traces += nz; ag.hs_valid = 0; }
     sum_z += (lane == 0) ? (unsigned long long)nz : 0ull;
     __syncwarp();
@@ -494,7 +522,10 @@ __device__ __forceinline__ void ln_step(const DevPtrs& ptr, const DynParams& D, 
     // theta updates (L2 reductions) are ordered before re-reads: only the parity record and an overfull update table need them
     if (env < P.record_envs && !dbg_nofence) __threadfence();
     LPH(9);
-    if (env < P.record_envs) { if (RESIDENT) emit_record_res(ptr, hdr, env, ag, theta_a, ag.to_vars, lane); else emit_record_ool(ptr, g, env, ag, theta_a, ag.to_vars, lane); }
+    if (env < P.record_envs) {  // (the out-of-line writers get a copy of the pointers: see td_decision above)
+      const DevPtrs pc = ptr;
+      if (RESIDENT) emit_record_res(pc, hdr, env, ag, theta_a, ag.to_vars, lane); else emit_record_ool(pc, g, env, ag, theta_a, ag.to_vars, lane);
+    }
     if (stage == 0) {
       // the to-state becomes the from-state; Q(from, .) under the UPDATED theta (serial.cpp:55,60)
       if (lane < RLM_N_STATE_MAX + 3) { ag.prev_vars[lane] = ag.from_vars[lane]; ag.from_vars[lane] = ag.to_vars[lane]; }
@@ -502,11 +533,17 @@ __device__ __forceinline__ void ln_step(const DevPtrs& ptr, const DynParams& D, 
       if (lane == 0) { ag.prev_null = ag.null_from; ag.null_from = 0; ag.n_steps++; ag.ep_step++; ag.need_begin = 1; }
       steps_done++;
       LPH(13);
-      if (local_patch) ln_patch_local(ut, scaled, h.s[0], h.s[1], h.s[2], h.null_state, lane, V + (table ? RLM_MAX_ACTIONS * LN_VROW : 0));  // the last batch of updates
+      if (local_patch) patched |= ln_patch_local(ut, scaled, h.s[0], h.s[1], h.s[2], h.null_state, lane, V + (table ? RLM_MAX_ACTIONS * LN_VROW : 0));  // the last batch of updates
       LPH(14);
       __syncwarp();
+      // with no weight of the to-state patched, V holds the first evaluation's operands and its sums are Q(to, .) bit for
+      // bit: the warp skips them (about half of C1's steps).  (The timing build's no-patch what-if always sums again.)
+      const bool again = __any_sync(FULL, patched) || !local_patch;
+#ifdef RLM_TIMING
+      if (lane == 0 && tp_idx < 4096) g_phase_clk[tp_idx * 16 + 15] = again;
+#endif
       LPH(10);
-      q = ln_sums(V, DBL, lane);
+      if (again) q = ln_sums(V, DBL, lane);
       ln_store_q<DBL>(ag, q, lane);
       LPH(11);
     }
