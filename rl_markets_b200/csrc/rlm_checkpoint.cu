@@ -290,6 +290,7 @@ struct CkHeader {
   DynParams shared_dyn;
 };
 static_assert(offsetof(CkHeader, model_log_cap) == 40 && offsetof(CkHeader, cfg) == 48, "lib.py reads the header at fixed offsets");
+static_assert(offsetof(CkHeader, library_fp) == 48 + sizeof(rlm_config) + 56, "tests/checkpoint_format.py reads library_fp after the config");
 struct CkSection { uint32_t id, table; uint64_t offset, bytes, count; };  // count: values of a packed table
 enum { CK_ENV = 1, CK_HSUM, CK_OCC, CK_TRACE_F, CK_TRACE_E, CK_MT_POL, CK_MT_AGT, CK_COUNTERS, CK_READY, CK_READY_COUNT, CK_RECORDS,
        CK_RECORD_COUNT, CK_TAPE_CUR, CK_TAPE_LO, CK_ENV_DAY, CK_DAY_OFF, CK_DAY_MARKET, CK_MARKETS, CK_ENV_MARKET, CK_REC_FIXED,

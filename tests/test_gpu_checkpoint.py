@@ -61,7 +61,7 @@ class Setup:
         self.cfg, self.env, self.library, self.day_markets, self.model_log = cfg, env or {}, library, day_markets, model_log
 
     def make(self, monkeypatch, env=None, fresh=False):
-        for k in ("RLM_ROUNDS", "RLM_ENV_VARIANT", "RLM_AGENT_VARIANT", "RLM_GRAPHS"):
+        for k in ("RLM_ROUNDS", "RLM_ENV_VARIANT", "RLM_AGENT_VARIANT", "RLM_GRAPHS", "RLM_SUBBATCHES"):
             monkeypatch.delenv(k, raising=False)
         for k, v in (self.env if env is None else env).items():
             monkeypatch.setenv(k, v)

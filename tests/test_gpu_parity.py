@@ -201,6 +201,7 @@ def test_stream_mode_in_short_run_calls(rlm, monkeypatch, env_vars, call_ticks):
     ({"RLM_ROUNDS": "0"}, "q_learn"),             # tick-synchronous engine for every call (long calls default to rounds)
     ({"RLM_ROUNDS": "0"}, "double_q_learn"),
     ({"RLM_ROUNDS": "1"}, "r_learn"),             # (not part of the default: R-learning stays tick-synchronous)
+    ({"RLM_SUBBATCHES": "3", "RLM_ROUNDS": "0"}, "q_learn"),  # three sub-batch streams; 5 envs fill the first, two stay empty
 ])
 def test_every_engine_variant_matches_oracle(rlm, oracle, monkeypatch, env_vars, algo):
     """The non-default kernels (selected by environment variables read in rlm_create) are held to the same bar."""
@@ -216,6 +217,25 @@ def test_every_engine_variant_matches_oracle(rlm, oracle, monkeypatch, env_vars,
         recs, _keep = m.records(b)
         assert len(recs) == port["steps"] > 100
         _compare_env(recs, port, "%s %r env %d" % (algo, env_vars, b))
+        assert bytes(m.theta(b, 0)) == bytes((C.c_double * M)(*port["theta"]))
+    m.close()
+
+
+def test_sub_batches_of_one_env_match_oracle(rlm, oracle, monkeypatch):
+    """RLM_SUBBATCHES=3 at 65 envs: split_batch cuts whole warps, so the sub-batches hold 32, 32 and 1 envs; the envs at
+    each sub-batch's edges are held to the oracle"""
+    monkeypatch.setenv("RLM_SUBBATCHES", "3")
+    monkeypatch.setenv("RLM_ROUNDS", "0")
+    n_envs, n_ticks, M = 65, 1500, 8192
+    y, cfg = _mk("q_learn", M, n_envs, flow_seed=23, rec_cap=800)
+    m = rlm.BatchedMarket(cfg)
+    m.run_ticks(n_ticks)
+    m.sync()
+    for b in (0, 31, 32, 63, 64):
+        port = oracle.run_port(cfg, b, oracle.generate_ticks(cfg, b, n_ticks))
+        recs, _keep = m.records(b)
+        assert len(recs) == port["steps"] > 100
+        _compare_env(recs, port, "sub-batches env %d" % b)
         assert bytes(m.theta(b, 0)) == bytes((C.c_double * M)(*port["theta"]))
     m.close()
 
